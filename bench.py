@@ -3,15 +3,16 @@
 
     python bench.py --gpus 1 --steps 3 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
-    python bench.py --impl reference ...        # the reference's own classes on the host cores (baseline/_ref), same metric
+    python bench.py --impl reference ...        # the reference's own classes on the host cores (oracle/_ref), same metric
 
-Workload (BASELINE.json configs[2]; SURVEY.md 8d item 3): full ABC cascade, batch 256 per GPU, S0 = 50 -> S = 100 faces,
-E = 40 edges/face (edge-stage sequences of 4000 tokens), dense masks, random-init weights, Gaussian inputs.
+Workload (BASELINE.json configs[2]; SURVEY.md 8d item 3): full ABC cascade, batch 64 per GPU (chosen for run time;
+--batch 256 also fits in 80 GB), S0 = 50 -> S = 100 faces, E = 40 edges/face (edge-stage sequences of 4000 tokens),
+dense masks, random-init weights, Gaussian inputs.
 One bench "step" = one pass of the whole cascade (SurfPos -> SurfZ -> EdgePos -> EdgeZ, every stage a DDPM loop of
 T = --steps-per-stage network evaluations + fused scheduler updates, then both VAE decodes when available) over one batch.
 Every DDPM step of a stage costs the same work whatever its t, so the metric (defined at T = 1000) is reported as
     value = n_gpus * B / (seconds_per_step * 1000 / T)
-with T stated in `config`; `--steps-per-stage 1000` runs the literal thing (minutes per step at B = 256).
+with T stated in `config`; `--steps-per-stage 1000` runs the literal thing (minutes per step at B = 64).
 Weak scaling: every rank runs its own batch of B; no collective on the hot path.
 """
 from __future__ import annotations
@@ -40,7 +41,7 @@ def parse():
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
-    ap.add_argument("--batch", type=int, default=256, help="B-reps per GPU")
+    ap.add_argument("--batch", type=int, default=64, help="B-reps per GPU")
     ap.add_argument("--surfaces", type=int, default=50)
     ap.add_argument("--edges", type=int, default=40)
     ap.add_argument("--steps-per-stage", type=int, default=4)
@@ -58,15 +59,20 @@ def parse():
                          "1000-step DDPM, 30 face tokens, batch 64 (first stage only), eager loop vs CUDA-graph replay")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's outputs as DIR/<name>.npy (float32, at most "
+                         "64 MB in all: a fixed, seeded sample of the batch when they are larger), so that two builds can "
+                         "be compared output for output")
     return ap.parse_args()
 
 
 def peaks():
+    """dense FP16/BF16 tensor peak of the H100 SXM (NVIDIA data sheet, 700 W); MEASURED_PEAKS.json overrides it"""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops", 1590.0), d.get("bf16_tflops_sustained", 1400.0), "measured"
-    return 1590.0, 1400.0, "fallback"
+        return d.get("bf16_tflops", 989.0), d.get("bf16_tflops_sustained", 989.0), "measured"
+    return 989.0, 989.0, "data sheet"
 
 
 # ------------------------------------------------------------------------------------------------ algorithmic FLOPs
@@ -105,7 +111,7 @@ def cpu_reference_sample(S0, S, E, reps, threads=None, inner_warm=True, kind="au
     step at batch 1, `reps` timed repetitions after one warm-up; extrapolated to the 4 x 1000-step cascade.
 
     kind = "reference": the reference's OWN classes (SurfPosNet ... EdgeZNet of network.py:1066-1393, stock code path:
-    nn.TransformerEncoder etc., eval(), no_grad), imported unmodified from baseline/_ref/network.py (or /root/reference)
+    nn.TransformerEncoder etc., eval(), no_grad), imported unmodified from oracle/_ref/network.py (or $BREPGEN_REFERENCE)
     through oracle/reference_loader.py; "port": oracle/denoisers.py (the pinned restatement); "auto": the reference when
     its file is present, else the port.  The scheduler step is oracle/schedulers.py in both cases (diffusers is absent
     offline; the step is < 0.1 % of the time).  Returns (B-reps/s, cores, description, kind_used)."""
@@ -119,7 +125,7 @@ def cpu_reference_sample(S0, S, E, reps, threads=None, inner_warm=True, kind="au
     torch.set_num_threads(cores)
     net = load_reference_network(required=False) if kind in ("auto", "reference") else None
     if kind == "reference" and net is None:
-        raise RuntimeError("reference classes requested but neither baseline/_ref/network.py nor /root/reference exists")
+        raise RuntimeError("reference classes requested but neither oracle/_ref/network.py nor $BREPGEN_REFERENCE exists")
     used = "reference" if net is not None else "port"
     ref_cls = None if net is None else {"surfpos": net.SurfPosNet, "surfz": net.SurfZNet, "edgepos": net.EdgePosNet,
                                         "edgez": net.EdgeZNet}
@@ -179,6 +185,25 @@ def best_cpu_threads():
         if best_t is None or dt < best_t:
             best, best_t = k, dt
     return best
+
+
+# ------------------------------------------------------------------------------------------------ output dump
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out, directory, budget=DUMP_BYTES):
+    """every output of the cascade (all batch-leading) as float32 .npy; when they exceed `budget` together, the same fixed,
+    seeded sample of batch rows (sorted) is kept from each, and its indices are written as batch_index.npy"""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    B = next(iter(out.values())).shape[0]
+    per_row = sum(v[0].numel() * 4 for v in out.values())
+    keep = max(1, min(B, (budget - 8 * B - (64 << 10)) // per_row))     # 64 KB for the .npy headers
+    idx = torch.arange(B) if keep == B else torch.randperm(B, generator=torch.Generator().manual_seed(0))[:keep].sort().values
+    for k, v in out.items():
+        np.save(os.path.join(directory, f"{k}.npy"), v.detach()[idx.to(v.device)].float().cpu().numpy())
+    if keep < B:
+        np.save(os.path.join(directory, "batch_index.npy"), idx.numpy())
 
 
 # ------------------------------------------------------------------------------------------------ clocks sampler
@@ -259,7 +284,7 @@ def run_surfpos(args):
     from brepgen_b200.synth import synth_state_dict
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
-    B, S, T = (args.batch if args.batch != 256 else 64), 30, 1000
+    B, S, T = args.batch, 30, 1000
     m = NETS["surfpos"](False)
     m.load_state_dict(synth_state_dict(denoiser_spec("surfpos", False), seed=1))
     casc = Cascade({"surfpos": m.to(dev).eval()}, device=dev)
@@ -291,6 +316,8 @@ def run_surfpos(args):
 
 def main():
     args = parse()
+    if args.dump_outputs and (args.impl == "reference" or args.workload != "cascade"):
+        sys.exit("bench.py: --dump-outputs writes the outputs of the cascade workload of this implementation only")
     if args.impl == "reference":
         return run_reference(args)
     if args.workload == "surfpos":
@@ -373,6 +400,8 @@ def main():
     ms = timed(step_resident, args.steps)
     launches = _ffi.lib().bg_launch_count() + _ffi.replayed_launches - l0      # host launches + kernels inside graph replays
     clk = clocks.finish()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(last["out"], args.dump_outputs)
     scale = 1000.0 / T if args.schedule == "ddpm" else 1.0     # the shipped hybrid is run literally
     # the two VAE decodes run once per cascade whatever T is: time them alone and keep them out of the 1000/T scaling
     ms_dec = 0.0
@@ -439,15 +468,9 @@ def main():
     fl_attn = B * 3072.0 * L * L
     ach = fl_attn / (ms_attn / 1e3) / 1e12
     del qkv, ao
-    traffic = None   # dram__bytes_read.sum + dram__bytes_write.sum of this kernel at this shape (ncu --set full capture)
-    tp = os.path.join(ROOT, "profiles", "attn_traffic.json")
-    if os.path.exists(tp):
-        tj = json.load(open(tp))
-        if tj.get("B") == B and tj.get("L") == L:
-            traffic = tj["dram_bytes_per_launch"]
-    roofline = {"bound": "tensor", "kernel": "attn_kernel<2> (tcgen05 flash attention, B=%d L=%d)" % (B, L),
+    roofline = {"bound": "tensor", "kernel": "attn_kernel (wgmma flash attention, B=%d L=%d)" % (B, L),
                 "achieved": ach, "peak": burst, "unit": "TFLOP/s", "frac": ach / burst, "peak_source": f"bf16_tflops burst, {src}",
-                "traffic": traffic, "ms_per_launch": ms_attn, "flop_per_launch": fl_attn}
+                "ms_per_launch": ms_attn, "flop_per_launch": fl_attn}
     # CFG doubles every forward; the shipped hybrid runs 158 PNDM + 250 DDPM forwards per stage (sample.py:128-155)
     flops_brep = cascade_flops_per_brep(S0, S, E, steps=1000 if args.schedule == "ddpm" else 408) * (2 if args.cf else 1)
     whole = {"algorithmic_tflop_per_brep": flops_brep / 1e12, "achieved_tflops_per_gpu": value / world * flops_brep / 1e12,
@@ -470,13 +493,13 @@ def main():
     if rank == 0:
         line = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
                 "ms_per_step": ms, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-                "dtype": "f16 x f16 -> f32 (tcgen05 kind::f16; split hi+lo weights on in/out-proj; fp32 residual/LN/softmax)",
+                "dtype": "f16 x f16 -> f32 (wgmma; split hi+lo weights on in/out-proj; fp32 residual/LN/softmax)",
                 "data": "synthetic",
                 "config": {"workload": f"{'furniture_cfg' if args.cf else 'abc'}_cascade B={B}/GPU S0={S0}->S={S} E={E} L_edge={L}, "
                                        f"{args.masks} masks, schedule={args.schedule}",
                            "ddpm_steps_per_stage_timed": T, "value_normalised_to_steps_per_stage": 1000,
                            "vae_decode_in_step": surf_vae is not None, "vae_decode_ms_per_step": ms_dec,
-                           "l2": "activations of one step (GBs) exceed the 126 MB L2; no explicit flush",
+                           "l2": "activations of one step (GBs) exceed the 50 MB L2; no explicit flush",
                            "precision": models["surfpos"].precision, "token_compaction": bool(args.compact), "parallelism": f"batch-sharded x{world}, no collective"},
                 "roofline": roofline, "whole_cascade": whole, "cpu_baseline": cpu, "e2e": e2e, "gpu_launches": int(launches),
                 "clocks": clk}

@@ -1,6 +1,6 @@
 """ctypes binding of libbrepgen_b200.so (the C ABI in include/brepgen_b200.h).
 
-The product path has NO fallback: if the shared library is missing or the device is not sm_100, calls raise.
+The product path has NO fallback: if the shared library is missing or the device is not sm_90 (H100), calls raise.
 """
 from __future__ import annotations
 

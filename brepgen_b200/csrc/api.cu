@@ -20,8 +20,8 @@ int bg_check_device(void) {
   BG_CUDA(cudaGetDevice(&dev));
   BG_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
   BG_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
-  if (major != 10)
-    return set_error(BG_ERR_UNSUPPORTED_ARCH, "brepgen_b200 kernels are built for sm_100a only; device is sm_" +
+  if (major != 9 || minor != 0)
+    return set_error(BG_ERR_UNSUPPORTED_ARCH, "brepgen_b200 kernels are built for sm_90a (H100) only; device is sm_" +
                                                   std::to_string(major) + std::to_string(minor));
   return BG_OK;
 }

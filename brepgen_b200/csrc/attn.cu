@@ -1,32 +1,22 @@
-// tcgen05 flash attention for the denoisers' self-attention (12 heads x 64, key-padding mask).
+// wgmma flash attention for the denoisers' self-attention (12 heads x 64, key-padding mask).
 //
 // Reference semantics: nn.MultiheadAttention inside nn.TransformerEncoderLayer with src_key_padding_mask
-// (/root/reference/network.py:1119-1123, 1193-1197, 1279-1283, 1387-1390): softmax(q k^T / 8 + (-inf on padded keys)) v.
+// (network.py:1119-1123, 1193-1197, 1279-1283, 1387-1390): softmax(q k^T / 8 + (-inf on padded keys)) v.
 // Edge stages run ONE sequence of L = faces*edges <= 4000 tokens per sample (network.py:1265-1283), so this is an
 // online-softmax (flash) kernel; the surface stages (L <= 100) use the same kernel with one key block.
 //
-// CTA = NT query tiles of 128 rows for one (sample, head):
-//   warps [0, 4*NT)   : softmax warpgroups, one per query tile; thread r owns query row r == TMEM lane r
-//   warp 4*NT         : TMA producer (Q once; K / V 128-key tiles through an ST-deep mbarrier ring)
-//   warps 4*NT+1 ..   : one MMA-issuing thread per query tile (the first of these warps owns the TMEM allocation)
-//   warps 12, 13 (HW) : helper warps: wait on the S-ready / PV-done mbarriers ahead of time and release the softmax
-//                       warpgroup of their tile through named barriers
-// per key block j and tile t:   S_t = Q_t K_j^T            4 x tcgen05.mma M128 N128 K16  (A,B K-major SW128)
-//                               P_t = exp2(c (S_t - m))     softmax WG: TMEM -> regs -> fp16 -> TMEM (tcgen05.st, 8 columns =
-//                                                           16 keys at a time, as produced)
-//                               O_t (+)= P_t V_j            8 x tcgen05.mma M128 N64 K16   (A = P from TMEM, B = V MN-major SW128)
-//                               O_t += P_t V_j accumulates in TMEM; lazy rescale of O_t by the softmax WG
-// MMA issue order  QK(0,j) QK(1,j) PV(0,j-1) PV(1,j-1)  lets softmax of block j overlap the PV of block j-1.
-// Round 2: P goes to tensor memory instead of shared memory (PT = 1, default for L > 128).  The P round trip through shared
-// memory was half of the kernel's shared-memory traffic (64 KB written + 64 KB read of 256 KB per key block and CTA) and each
-// block paid a generic->async proxy fence after its 16 STS.128; with P in TMEM the stores are 8 tcgen05.st.x8 issued as the
-// groups are produced and the release is a tcgen05 fence: 719 -> 797 TF/s at B = 64, 675 -> 754 at B = 256 (measured,
-// profiles/r02_attention_experiments.md, which also lists what did NOT help: half-tile P hand-over, speculative reference
-// with the row max inside the exponential loop, XU token with a data dependency, deferred proxy fence).
+// CTA = one 128-row query tile of one (sample, head), 384 threads = 3 warpgroups:
+//   warpgroup 0    : TMA producer (one elected thread: Q once; K / V 128-key tiles through an ST-deep mbarrier ring);
+//                    gives its registers to the consumers (setmaxnreg)
+//   warpgroups 1-2 : consumers, 64 query rows each; per key block j:
+//                      S = Q K_j^T          4 x wgmma m64n128k16, Q and K K-major SW128 from shared memory
+//                      P = exp2(c (S - m))  in registers (fp32 online softmax, rows split over lane quads)
+//                      O = O a + P V_j      8 x wgmma m64n64k16, A = P as fp16 straight from the S registers,
+//                                           B = V MN-major SW128 from shared memory
+//                    S, P and O never leave the registers; the two consumer warpgroups interleave on the tensor core.
 // Fully padded key blocks are skipped through a per-sample block list (result-preserving: their p is exactly 0).
 // Roofline: tensor-bound; 4*L*L*64 flop per (sample, head).
 #include <math.h>
-#include <stdlib.h>
 
 #include "bg_internal.h"
 #include "ptx.cuh"
@@ -39,26 +29,18 @@ namespace {
 constexpr int DH = 64;
 constexpr int NHEAD = 12;
 constexpr int DMODEL = 768;
+constexpr int BQ = 128;                    // query rows per CTA (two consumer warpgroups of 64)
 constexpr int TILE_BYTES = 128 * DH * 2;   // 16 KB: Q / K / V tile, 128 rows x 128 B
-constexpr int P_BYTES = 128 * 128 * 2;     // 32 KB: two K-major SW128 blocks of 64 keys
-
-template <int NT>
-struct ACfg {
-  static constexpr int ST = (NT == 2) ? 3 : 2;              // K / V ring depth
-  static constexpr int PB = 1;                              // P buffers per tile
-  static constexpr int OFF_Q = 0;
-  static constexpr int OFF_K = NT * TILE_BYTES;
-  static constexpr int OFF_V = OFF_K + ST * TILE_BYTES;
-  static constexpr int OFF_P = OFF_V + ST * TILE_BYTES;
-  static constexpr int OFF_BAR = OFF_P + NT * PB * P_BYTES;
-  static constexpr int OFF_MASKW = OFF_BAR + 512;          // invalid-key bit words: 4 per key block, MAX_KB blocks
-  static constexpr int MAX_KB = 64;                        // L <= 8192
-  static constexpr int SMEM_BYTES = OFF_MASKW + MAX_KB * 16 + 1024;
-  static constexpr int TMEM_COLS = (NT == 2) ? 512 : 256;
-  // NT == 2: three full warpgroups (2 softmax + 1 for the producer / MMA warps) so setmaxnreg can move registers
-  static constexpr int THREADS = (NT == 2) ? 384 : NT * 128 + 64;
-  static constexpr int TILE_COLS = 256;   // per tile: S at +0 (128 cols), O at +128 (64), P (fp16 pairs, PT mode) at +192 (64)
-};
+constexpr int ST = 2;                      // K / V ring depth
+constexpr int OFF_Q = 0;
+constexpr int OFF_K = TILE_BYTES;
+constexpr int OFF_V = OFF_K + ST * TILE_BYTES;
+constexpr int OFF_BAR = OFF_V + ST * TILE_BYTES;
+constexpr int OFF_MASKW = OFF_BAR + 256;   // invalid-key bit words: 4 per key block, MAX_KB blocks
+constexpr int MAX_KB = 64;                 // L <= 8192
+constexpr int SMEM_BYTES = OFF_MASKW + MAX_KB * 16 + 1024;
+constexpr int THREADS = 384;
+constexpr int CONSUMER_THREADS = 256;
 
 struct AttnParams {
   __half* out;
@@ -70,53 +52,32 @@ struct AttnParams {
   const uint32_t* blk_words;   // [B][nkb][4] invalid-key bit words of the listed blocks, list order (per forward), or null
   const int* seq_row0;         // variable-length mode: first row / number of rows of every sample, or null (dense)
   const int* seq_len;
-  float scale_log2;   // log2(e) / sqrt(64)
-  int pingpong;       // XU token between the two softmax warpgroups (named barriers)
-  int probe;          // early non-blocking mbarrier probes
+  float scale_log2;            // log2(e) / sqrt(64)
 };
 
-// -DBG_ATTN_TRACE (`make trace`, tools/attn_trace.py): clock64 stamps of the softmax thread of row 0 of both tiles of one CTA
-#ifdef BG_ATTN_TRACE
-__device__ long long g_attn_trace[2][64][8];
-#define BG_TR(pt)                                                                                                    \
-  do {                                                                                                               \
-    if ((threadIdx.x & 127) == 0 && blockIdx.x == 3 && blockIdx.y == 5 && blockIdx.z == 1 && it < 64)                \
-      g_attn_trace[t][it][pt] = clock64();                                                                           \
-  } while (0)
-#else
-#define BG_TR(pt)
-#endif
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
 
-// PM: which exponentials run as a polynomial on the FMA pipe instead of MUFU.EX2: bit q of the low byte = element pair q
-// (0..7) of the EVEN 16-key groups, of the high byte = of the odd groups (0x8888 = pairs 3 and 7 of every group = 25 %).
-// Dispatch costs measured in profiles/r02_pipe_rates.txt: a polynomial pair ~22 cycles of the sub-partition's dispatch
-// port, two MUFU ~5 (+ 16 cycles of the XU pipe, 16 ex2/clk/SM)
-// PT: P goes to TENSOR MEMORY (tcgen05.st, two fp16 per column) and the PV MMA takes its A operand from TMEM -- per key
-// block this removes 64 KB of shared-memory writes + 64 KB of reads, which otherwise make the kernel smem-bandwidth bound
-// (QK^T and PV operand reads + P + TMA fills = 256 KB per block ~ 2048 cycles at 128 B/clk vs 1024 MMA cycles).
-// HW: two extra "helper" warps (a 4th warpgroup, 512 threads) do the mbarrier waits for S-ready / PV-done ahead of time
-// and release the softmax warpgroups through named barriers: an mbarrier probe costs ~150-230 cycles of latency on the
-// softmax critical path even when the phase completed long ago, a named-barrier sync ~15.
-template <int NT, int PM, int PT, int HW>
-__global__ void __launch_bounds__(HW ? 512 : ACfg<NT>::THREADS, (NT == 2) ? 1 : 2)
+__global__ void __launch_bounds__(THREADS, 1)
 attn_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParams p) {
-  using C = ACfg<NT>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
   uint64_t* q_full = bars;
   uint64_t* k_full = q_full + 1;
-  uint64_t* k_empty = k_full + C::ST;
-  uint64_t* v_full = k_empty + C::ST;
-  uint64_t* v_empty = v_full + C::ST;
-  uint64_t* s_full = v_empty + C::ST;
-  uint64_t* s_free = s_full + NT;
-  uint64_t* p_full = s_free + NT;
-  uint64_t* pv_full = p_full + NT;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(pv_full + NT * C::PB);   // pv_full[t * PB + (block % PB)]
+  uint64_t* k_empty = k_full + ST;
+  uint64_t* v_full = k_empty + ST;
+  uint64_t* v_empty = v_full + ST;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
   const int qgrp = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   // QKV / out are addressed as ONE [rows][cols] matrix; sample b owns rows [row0, row0 + len).  Dense: row0 = b * L, len = L.
   // Variable-length mode (mask-aware token compaction): rows of the valid tokens only, packed back to back.  A tile may then
@@ -124,347 +85,169 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParams p) {
   // are never written.
   const int row0 = p.seq_row0 ? p.seq_row0[b] : b * p.L;
   const int len = p.seq_len ? p.seq_len[b] : p.L;
-  if (qgrp * NT * 128 >= len) return;     // variable-length mode: the grid is sized for the longest sample
+  if (qgrp * BQ >= len) return;     // variable-length mode: the grid is sized for the longest sample
   const int nblk = p.blk_count ? p.blk_count[b] : (len + 127) / 128;
   const int* blist = p.blk_list ? p.blk_list + (size_t)b * p.nkb : nullptr;
 
-  constexpr int PRODUCER_WARP = NT * 4;
-  constexpr int MMA_WARP = NT * 4 + 1;
-
-  if (warp == PRODUCER_WARP && elect_one()) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQKV);
     mbar_init(q_full, 1);
-    for (int i = 0; i < C::ST; ++i) {
+    for (int i = 0; i < ST; ++i) {
       mbar_init(&k_full[i], 1);
-      mbar_init(&k_empty[i], NT);     // one tcgen05.commit per MMA-issuing thread (one thread per query tile)
+      mbar_init(&k_empty[i], CONSUMER_THREADS);
       mbar_init(&v_full[i], 1);
-      mbar_init(&v_empty[i], NT);
-    }
-    for (int t = 0; t < NT; ++t) {
-      mbar_init(&s_full[t], 1);
-      mbar_init(&s_free[t], 128);
-      mbar_init(&p_full[t], 128);
-      for (int i = 0; i < C::PB; ++i) mbar_init(&pv_full[t * C::PB + i], 1);
+      mbar_init(&v_empty[i], CONSUMER_THREADS);
     }
     fence_barrier_init();
-    // start the first loads right away (this thread initialised the barriers itself): they overlap with the TMEM
-    // allocation, the mask-word construction and the CTA-wide synchronisation below
-    mbar_arrive_expect_tx(q_full, NT * TILE_BYTES);
-    for (int t = 0; t < NT; ++t)
-      tma_load_2d(smem + C::OFF_Q + t * TILE_BYTES, &tmQKV, q_full, h * DH, row0 + (qgrp * NT + t) * 128);
-    for (int it = 0; it < nblk && it < C::ST; ++it) {
-      const int kb = blist ? blist[it] : it;
-      mbar_arrive_expect_tx(&k_full[it], TILE_BYTES);
-      tma_load_2d(smem + C::OFF_K + it * TILE_BYTES, &tmQKV, &k_full[it], DMODEL + h * DH, row0 + kb * 128);
-      mbar_arrive_expect_tx(&v_full[it], TILE_BYTES);
-      tma_load_2d(smem + C::OFF_V + it * TILE_BYTES, &tmQKV, &v_full[it], 2 * DMODEL + h * DH, row0 + kb * 128);
-    }
   }
-  if (warp == MMA_WARP) tmem_alloc<C::TMEM_COLS>(tmem_slot);
-  // invalid-key bit words for every key block this CTA will visit (padded key or key >= L), built once: keeps the
+  // invalid-key bit words for every key block this CTA will visit (padded key or key >= len), built once: keeps the
   // global mask bytes off the per-block critical path
-  uint32_t* maskw = reinterpret_cast<uint32_t*>(smem + C::OFF_MASKW);
-  if (warp < PRODUCER_WARP) {
-    if (p.blk_words || !p.key_mask) {
-      // one word per thread, no dependent global-load chain: either copied from the per-forward table or, without a
-      // mask, computed (only keys >= L are invalid)
-      for (int wi = threadIdx.x; wi < nblk * 4; wi += PRODUCER_WARP * 32) {
-        uint32_t w;
-        if (p.blk_words) {      // list order: entry wi >> 2 belongs to key block blist[wi >> 2]
-          w = p.blk_words[((size_t)b * p.nkb + (wi >> 2)) * 4 + (wi & 3)];
-        } else {
-          const int base = (wi >> 2) * 128 + (wi & 3) * 32;
-          w = base + 32 <= len ? 0u : (base >= len ? 0xffffffffu : (0xffffffffu << (len - base)));
-        }
-        maskw[wi] = w;
+  uint32_t* maskw = reinterpret_cast<uint32_t*>(smem + OFF_MASKW);
+  if (p.blk_words || !p.key_mask) {
+    // one word per thread, no dependent global-load chain: either copied from the per-forward table or, without a
+    // mask, computed (only keys >= len are invalid)
+    for (int wi = threadIdx.x; wi < nblk * 4; wi += THREADS) {
+      uint32_t w;
+      if (p.blk_words) {      // list order: entry wi >> 2 belongs to key block blist[wi >> 2]
+        w = p.blk_words[((size_t)b * p.nkb + (wi >> 2)) * 4 + (wi & 3)];
+      } else {
+        const int base = (wi >> 2) * 128 + (wi & 3) * 32;
+        w = base + 32 <= len ? 0u : (base >= len ? 0xffffffffu : (0xffffffffu << (len - base)));
       }
-    } else {
-      for (int wi = warp; wi < nblk * 4; wi += PRODUCER_WARP) {
-        const int kb = blist ? blist[wi >> 2] : (wi >> 2);
-        const int key = kb * 128 + (wi & 3) * 32 + lane;
-        bool bad = key >= len;
-        if (!bad && p.key_mask) bad = p.key_mask[(size_t)b * p.L + key] != 0;
-        const uint32_t w = __ballot_sync(0xffffffffu, bad);
-        if (lane == 0) maskw[wi] = w;
-      }
+      maskw[wi] = w;
+    }
+  } else {
+    for (int wi = warp; wi < nblk * 4; wi += THREADS / 32) {
+      const int kb = blist ? blist[wi >> 2] : (wi >> 2);
+      const int key = kb * 128 + (wi & 3) * 32 + lane;
+      bool bad = key >= len;
+      if (!bad) bad = p.key_mask[(size_t)b * p.L + key] != 0;
+      const uint32_t w = __ballot_sync(0xffffffffu, bad);
+      if (lane == 0) maskw[wi] = w;
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // register rebalancing (NT == 2): the softmax warpgroups hold a 128-wide score row per thread; the third warpgroup
-  // (producer, MMA issuer, two idle warps) gives its registers away.  Each role sets its budget inside its own branch.
-  if (warp >= PRODUCER_WARP) {
-   if constexpr (NT == 2 && HW) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-   else if constexpr (NT == 2) asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
-   if (HW && warp >= 12 && warp < 12 + NT) {
-    // helper warp of tile t: named barrier 3 + t = "S_t of this block is in TMEM", 5 + t = "PV_t of the previous block done"
-    const int t = warp - 12;
-    for (int it = 0; it < nblk; ++it) {
-      mbar_wait(&s_full[t], it & 1);
-      named_bar_arrive(3 + t, 160);
-      if (it > 0) {
-        mbar_wait(&pv_full[t * C::PB], (it - 1) & 1);
-        named_bar_arrive(5 + t, 160);
-      }
-    }
-    if (nblk > 0) {
-      mbar_wait(&pv_full[t * C::PB], (nblk - 1) & 1);
-      named_bar_arrive(5 + t, 160);
-    }
-   } else
-   if (warp == PRODUCER_WARP) {
-    if (elect_one()) {
-      for (int it = C::ST; it < nblk; ++it) {       // the first ST blocks were issued before the CTA-wide sync
+  if (wg == 0) {
+    setmaxnreg_dec<24>();
+    if (warp == 0 && elect_one()) {
+      mbar_arrive_expect_tx(q_full, TILE_BYTES);
+      tma_load_2d(smem + OFF_Q, &tmQKV, q_full, h * DH, row0 + qgrp * BQ);
+      for (int it = 0; it < nblk; ++it) {
         const int kb = blist ? blist[it] : it;
-        const int s = it % C::ST;
-        const uint32_t par = ((it / C::ST) & 1) ^ 1;
+        const int s = it % ST;
+        const uint32_t par = ((it / ST) & 1) ^ 1;
         mbar_wait(&k_empty[s], par);
         mbar_arrive_expect_tx(&k_full[s], TILE_BYTES);
-        tma_load_2d(smem + C::OFF_K + s * TILE_BYTES, &tmQKV, &k_full[s], DMODEL + h * DH, row0 + kb * 128);
+        tma_load_2d(smem + OFF_K + s * TILE_BYTES, &tmQKV, &k_full[s], DMODEL + h * DH, row0 + kb * 128);
         mbar_wait(&v_empty[s], par);
         mbar_arrive_expect_tx(&v_full[s], TILE_BYTES);
-        tma_load_2d(smem + C::OFF_V + s * TILE_BYTES, &tmQKV, &v_full[s], 2 * DMODEL + h * DH, row0 + kb * 128);
+        tma_load_2d(smem + OFF_V + s * TILE_BYTES, &tmQKV, &v_full[s], 2 * DMODEL + h * DH, row0 + kb * 128);
       }
     }
-   } else if (warp < MMA_WARP + NT) {
-    // one MMA-issuing thread per query tile: the two softmax warpgroups are not coupled through one in-order issuer
-    if (elect_one()) {
-      const int t = warp - MMA_WARP;
-      constexpr uint32_t idesc_qk = make_idesc_f16(128, 128, 0, 0);
-      constexpr uint32_t idesc_pv = make_idesc_f16(128, DH, 0, 1);   // B (= V) is MN-major
-      mbar_wait(q_full, 0);
-      tc_fence_after();
-      for (int it = 0; it <= nblk; ++it) {
-        if (it < nblk) {
-          const int s = it % C::ST;
-          mbar_wait(&k_full[s], (it / C::ST) & 1);
-          mbar_wait(&s_free[t], (it & 1) ^ 1);
-          tc_fence_after();
-          const uint32_t k_addr = smem_u32(smem + C::OFF_K + s * TILE_BYTES);
-          const uint32_t q_addr = smem_u32(smem + C::OFF_Q + t * TILE_BYTES);
-#pragma unroll
-          for (int k = 0; k < DH / 16; ++k)
-            umma_f16_ss(tmem_base + t * C::TILE_COLS, make_sw128_desc(q_addr + k * 32), make_sw128_desc(k_addr + k * 32),
-                        idesc_qk, k > 0 ? 1u : 0u);
-          umma_commit(&s_full[t]);
-          umma_commit(&k_empty[s]);
-        }
-        if (it > 0) {
-          const int i = it - 1;
-          const int s = i % C::ST;
-          mbar_wait(&v_full[s], (i / C::ST) & 1);
-          mbar_wait(&p_full[t], i & 1);       // P_t(i) written and O_t rescaled (if needed) by the softmax warpgroup
-          tc_fence_after();
-          const uint32_t v_addr = smem_u32(smem + C::OFF_V + s * TILE_BYTES);
-          const uint32_t p_addr = smem_u32(smem + C::OFF_P + (t * C::PB + i % C::PB) * P_BYTES);
-#pragma unroll
-          for (int k = 0; k < 128 / 16; ++k)
-            if (PT)   // A = P from TMEM: lane = query row, 8 columns (16 fp16) per K = 16 step
-              umma_f16_ts(tmem_base + t * C::TILE_COLS + 128, tmem_base + t * C::TILE_COLS + 192 + k * 8,
-                          make_sw128_desc(v_addr + k * 2048), idesc_pv, (i | k) != 0 ? 1u : 0u);
-            else
-              umma_f16_ss(tmem_base + t * C::TILE_COLS + 128,
-                          make_sw128_desc(p_addr + (k >> 2) * (P_BYTES / 2) + (k & 3) * 32),
-                          make_sw128_desc(v_addr + k * 2048), idesc_pv, (i | k) != 0 ? 1u : 0u);
-          umma_commit(&pv_full[t * C::PB + i % C::PB]);
-          umma_commit(&v_empty[s]);
-        }
-      }
-    }
-   }
-  } else {
-    if constexpr (NT == 2 && HW) asm volatile("setmaxnreg.inc.sync.aligned.u32 208;");
-    else if constexpr (NT == 2) asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
-    // ------------------------------------------------------------------ softmax warpgroup for query tile t
-    // One thread per query row (== TMEM lane).  The whole 128-key score row lives in registers (one TMEM read, S is
-    // released to the next QK^T right away); O accumulates in TMEM across key blocks and is rescaled lazily: the
-    // exponent reference m_ref only moves when the running max grew by more than 2^8 (p <= 256 is harmless in fp16 P /
-    // fp32 accumulation), so the TMEM read-modify-write of O is rare after the first blocks.
-    const int t = warp >> 2;
-    const int r = threadIdx.x & 127;                       // query row in tile == TMEM lane
-    const uint32_t lane_base = (uint32_t)((warp & 3) * 32) << 16;
-    const uint32_t s_tmem = tmem_base + lane_base + t * C::TILE_COLS;
-    const uint32_t o_tmem = s_tmem + 128;
-    const uint32_t sP0 = smem_u32(smem + C::OFF_P + t * C::PB * P_BYTES) + r * 128;
-    // PV(i) reads P buffer i % PB and completes on pv_full[t][i % PB] (its (i / PB)-th completion)
-    auto wait_pv = [&](int i) {
-      if (HW) named_bar_sync(5 + t, 160);
-      else mbar_wait(&pv_full[t * C::PB + i % C::PB], (i / C::PB) & 1);
-    };
-    const float c = p.scale_log2;
-
-    float m_ref = -INFINITY, l = 0.f;
-
-    // mbarrier probes cost ~150 cycles of latency even when the phase has long completed; they are therefore ISSUED
-    // early (non-blocking test_wait) and only CONSUMED where the data is needed, with a blocking wait as the fallback.
-    bool s_ready = false;
-    const bool pingpong = NT == 2 && p.pingpong != 0;
-    if (pingpong && t == 1 && nblk > 0) named_bar_arrive(1, 256);
-    for (int it = 0; it < nblk; ++it) {
-      const uint4 iw = *reinterpret_cast<const uint4*>(maskw + it * 4);
-      const uint32_t inval[4] = {iw.x, iw.y, iw.z, iw.w};
-
-      BG_TR(0);
-      if (HW) named_bar_sync(3 + t, 160);
-      else if (!s_ready) mbar_wait(&s_full[t], it & 1);
-      BG_TR(6);
-      tc_fence_after();
-      float s[128];
-#pragma unroll
-      for (int cc = 0; cc < 4; ++cc) tmem_ld_32x32b_x32(s_tmem + cc * 32, reinterpret_cast<uint32_t*>(s) + cc * 32);
-      // probe "PV of the previous block done" while the TMEM load is in flight (PB == 1: one barrier per tile)
-      bool pv_ready = it == 0;
-      if (!HW && it > 0 && p.probe) pv_ready = mbar_test_wait(&pv_full[t * C::PB + (it - 1) % C::PB], ((it - 1) / C::PB) & 1);
-      tmem_ld_wait();
-      BG_TR(1);
-      tc_fence_before();
-      mbar_arrive(&s_free[t]);          // S_t may be overwritten by QK^T of the next block
-
-      if ((inval[0] | inval[1] | inval[2] | inval[3]) != 0) {
-#pragma unroll
-        for (int i = 0; i < 128; ++i)
-          if ((inval[i >> 5] >> (i & 31)) & 1u) s[i] = -INFINITY;
-      }
-      float mx[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) mx[j] = fmaxf(s[2 * j], s[2 * j + 1]);
-#pragma unroll
-      for (int i = 16; i < 128; i += 16) {     // eight independent FMNMX3 chains
-#pragma unroll
-        for (int j = 0; j < 8; ++j) mx[j] = fmax3(mx[j], s[i + 2 * j], s[i + 2 * j + 1]);
-      }
-      const float m_new = fmaxf(fmax3(m_ref, fmax3(mx[0], mx[1], mx[2]), fmax3(mx[3], mx[4], mx[5])), fmaxf(mx[6], mx[7]));
-
-      if (it == 0) {
-        m_ref = (m_new == -INFINITY) ? 0.f : m_new;
-      } else {
-        const bool need = (m_new - m_ref) * c > 8.f;
-        if (__any_sync(0xffffffffu, need)) {
-          if (!pv_ready) wait_pv(it - 1); // O_t complete up to block it-1 before its read-modify-write
-          pv_ready = true;
-          tc_fence_after();
-          const float f = need ? ex2((m_ref - m_new) * c) : 1.f;
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
-            uint32_t rr[32];
-            tmem_ld_32x32b_x32(o_tmem + hh * 32, rr);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) rr[i] = __float_as_uint(__uint_as_float(rr[i]) * f);
-            tmem_st_32x32b_x32(o_tmem + hh * 32, rr);
-          }
-          tmem_st_wait();
-          l *= f;
-          if (need) m_ref = m_new;
-        }
-      }
-      BG_TR(2);
-      if (it >= C::PB && !pv_ready) wait_pv(it - C::PB);   // the PV MMA that read this P buffer has finished
-      // probe the next block's scores now; the answer is consumed at the top of the next iteration
-      s_ready = (!HW && p.probe && it + 1 < nblk) ? mbar_test_wait(&s_full[t], (it + 1) & 1) : false;
-      BG_TR(7);
-      if (pingpong) named_bar_sync(1 + t, 256);
-      BG_TR(3);
-      const uint32_t sP = sP0 + (it % C::PB) * P_BYTES;
-      const float2 c2 = make_float2(c, c);
-      const float2 nmc2 = make_float2(-m_ref * c, -m_ref * c);
-
-      // p = exp2(c s - c m_ref), row sum (packed f32x2 math), fp16 P into the K-major SW128 layout.
-      // Software-pipelined by one 16-key group: the 16 MUFU.EX2 of group g are issued back to back, and only then are
-      // the results of group g-1 summed, packed and stored -- a consumer placed right behind its MUFU would stall the
-      // (in-order) warp for the MUFU latency and leave the XU pipe idle.
-      float2 acc = make_float2(0.f, 0.f), acc1 = make_float2(0.f, 0.f);
-      float2 ecur[8], eprev[8];
-      auto exp_group = [&](int g, float2 (&e)[8]) {
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const float2 a = ffma2(make_float2(s[16 * g + 2 * q], s[16 * g + 2 * q + 1]), c2, nmc2);
-          // PM: bit q of the low byte = element pair q (0..7) of the even 16-key groups, of the high byte = of the odd groups
-          e[q] = ((PM >> ((g & 1) * 8 + q)) & 1) ? exp2_poly2(a) : make_float2(ex2(a.x), ex2(a.y));
-        }
-      };
-      auto drain_group = [&](int g, const float2 (&e)[8]) {
-        uint32_t pk8[8];
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          uint32_t pk[4];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const float2 v = e[4 * hh + q];
-            if (q & 1) acc1 = fadd2(acc1, v); else acc = fadd2(acc, v);
-            __half2 h = __floats2half2_rn(v.x, v.y);
-            pk[q] = *reinterpret_cast<uint32_t*>(&h);
-          }
-          const int j8 = 2 * g + hh;                         // 16-byte chunk (8 keys) index along the 128 keys
-          if (PT) {
-#pragma unroll
-            for (int q = 0; q < 4; ++q) pk8[4 * hh + q] = pk[q];
-          } else {
-            st_shared_v4(sP + (j8 >> 3) * (P_BYTES / 2) + (((j8 & 7) ^ (r & 7)) << 4), pk[0], pk[1], pk[2], pk[3]);
-          }
-        }
-        if (PT) tmem_st_32x32b_x8(s_tmem + 192 + 8 * g, pk8);   // 16 keys = 8 columns of packed fp16 pairs, as produced
-      };
-      exp_group(0, eprev);
-#pragma unroll
-      for (int g = 1; g < 8; ++g) {
-        exp_group(g, ecur);
-        drain_group(g - 1, eprev);
-#pragma unroll
-        for (int q = 0; q < 8; ++q) eprev[q] = ecur[q];
-      }
-      drain_group(7, eprev);
-      if (pingpong && !(t == 1 && it == nblk - 1)) named_bar_arrive(1 + (1 - t), 256);   // hand the XU token over
-      tc_fence_before();                // orders the (rare) O rescale before the PV MMA that p_full releases
-      if (PT) {
-        tmem_st_wait();
-        tc_fence_before();
-      } else {
-        fence_proxy_async_smem();       // generic-proxy writes of P -> visible to the tensor core (async proxy)
-      }
-      BG_TR(4);
-      mbar_arrive(&p_full[t]);
-      l += (acc.x + acc.y) + (acc1.x + acc1.y);
-      BG_TR(5);
-    }
-
-    float o[DH];
-    if (nblk > 0) {
-      wait_pv(nblk - 1);
-      tc_fence_after();
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) tmem_ld_32x32b_x32(o_tmem + hh * 32, reinterpret_cast<uint32_t*>(o) + hh * 32);
-      tmem_ld_wait();
-    } else {
-#pragma unroll
-      for (int i = 0; i < DH; ++i) o[i] = 0.f;
-    }
-    const int row = (qgrp * NT + t) * 128 + r;
-    if (row < len) {
-      const float inv = l > 0.f ? 1.f / l : 0.f;
-      uint4* dst = reinterpret_cast<uint4*>(p.out + ((size_t)row0 + row) * p.ldo + h * DH);
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        __half2 h0 = __floats2half2_rn(o[8 * q] * inv, o[8 * q + 1] * inv);
-        __half2 h1 = __floats2half2_rn(o[8 * q + 2] * inv, o[8 * q + 3] * inv);
-        __half2 h2 = __floats2half2_rn(o[8 * q + 4] * inv, o[8 * q + 5] * inv);
-        __half2 h3 = __floats2half2_rn(o[8 * q + 6] * inv, o[8 * q + 7] * inv);
-        uint4 u;
-        u.x = *reinterpret_cast<uint32_t*>(&h0);
-        u.y = *reinterpret_cast<uint32_t*>(&h1);
-        u.z = *reinterpret_cast<uint32_t*>(&h2);
-        u.w = *reinterpret_cast<uint32_t*>(&h3);
-        dst[q] = u;
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) tmem_dealloc<C::TMEM_COLS>(tmem_base);
+  setmaxnreg_inc<240>();
+  // ------------------------------------------------------------------ consumer warpgroup: 64 query rows
+  // Accumulator layout (wgmma m64nN, fp32): warp w of the warpgroup owns rows 16w + lane / 4 (elements 4i, 4i + 1) and
+  // 16w + 8 + lane / 4 (elements 4i + 2, 4i + 3), at columns 8i + 2 (lane % 4) + {0, 1}.  Every row is spread over one
+  // lane quad, so row statistics need two shuffles.
+  const int half = wg - 1;
+  const int wq = warp & 3;
+  const float c = p.scale_log2;
+  const uint32_t q_addr = smem_u32(smem + OFF_Q) + half * 64 * 128;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  float o[DH / 2];
+#pragma unroll
+  for (int i = 0; i < DH / 2; ++i) o[i] = 0.f;
+
+  mbar_wait(q_full, 0);
+  for (int it = 0; it < nblk; ++it) {
+    const int s = it % ST;
+    const uint32_t par = (it / ST) & 1;
+    float sc[64];
+    mbar_wait(&k_full[s], par);
+    const uint32_t k_addr = smem_u32(smem + OFF_K + s * TILE_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < DH / 16; ++k)
+      wgmma_m64n128k16_ss(sc, make_sw128_desc(q_addr + k * 32), make_sw128_desc(k_addr + k * 32), k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operand(sc);
+    mbar_arrive(&k_empty[s]);
+
+    const uint4 iw = *reinterpret_cast<const uint4*>(maskw + it * 4);
+    if ((iw.x | iw.y | iw.z | iw.w) != 0) {
+      const uint32_t inval[4] = {iw.x, iw.y, iw.z, iw.w};
+#pragma unroll
+      for (int i = 0; i < 16; ++i)
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const int key = 8 * i + 2 * (lane & 3) + j;
+          if ((inval[key >> 5] >> (key & 31)) & 1u) {
+            sc[4 * i + j] = -INFINITY;
+            sc[4 * i + 2 + j] = -INFINITY;
+          }
+        }
+    }
+    float ref[2], alpha[2];
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int i = 0; i < 16; ++i) mx = fmaxf(mx, fmaxf(sc[4 * i + 2 * hr], sc[4 * i + 2 * hr + 1]));
+      const float m_new = fmaxf(m_run[hr], quad_max(mx));
+      ref[hr] = m_new == -INFINITY ? 0.f : m_new;        // a row without any valid key so far keeps p = 0
+      alpha[hr] = ex2((m_run[hr] - ref[hr]) * c);         // 0 while the row had no valid key (m_run = -inf)
+      m_run[hr] = m_new;
+      l_run[hr] *= alpha[hr];
+    }
+#pragma unroll
+    for (int i = 0; i < DH / 8; ++i) {
+      o[4 * i] *= alpha[0];
+      o[4 * i + 1] *= alpha[0];
+      o[4 * i + 2] *= alpha[1];
+      o[4 * i + 3] *= alpha[1];
+    }
+    // p = exp2(c s - c m), row sums in fp32, and the fp16 A fragments of P V: the A fragment of key slice kk (16 keys)
+    // is {rows r, r + 8} x {keys 16kk + 2 (lane % 4) + {0, 1}, + 8}, i.e. exactly accumulator columns 2kk and 2kk + 1
+    uint32_t pa[8][4];
+    const float nm0 = -ref[0] * c, nm1 = -ref[1] * c;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const float p0 = ex2(fmaf(sc[4 * i], c, nm0)), p1 = ex2(fmaf(sc[4 * i + 1], c, nm0));
+      const float p2 = ex2(fmaf(sc[4 * i + 2], c, nm1)), p3 = ex2(fmaf(sc[4 * i + 3], c, nm1));
+      l_run[0] += p0 + p1;
+      l_run[1] += p2 + p3;
+      pa[i >> 1][(i & 1) * 2] = pack_half2(p0, p1);
+      pa[i >> 1][(i & 1) * 2 + 1] = pack_half2(p2, p3);
+    }
+
+    mbar_wait(&v_full[s], par);
+    const uint32_t v_addr = smem_u32(smem + OFF_V + s * TILE_BYTES);
+    wgmma_fence_operand(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) wgmma_m64n64k16_rs_bt(o, pa[kk], make_sw128_desc(v_addr + kk * 2048), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operand(o);
+    mbar_arrive(&v_empty[s]);
+  }
+
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const float l = quad_sum(l_run[hr]);
+    const float inv = l > 0.f ? 1.f / l : 0.f;
+    const int row = qgrp * BQ + half * 64 + wq * 16 + hr * 8 + (lane >> 2);
+    if (row >= len) continue;
+    __half* dst = p.out + ((size_t)row0 + row) * p.ldo + h * DH + 2 * (lane & 3);
+#pragma unroll
+    for (int i = 0; i < DH / 8; ++i)
+      *reinterpret_cast<uint32_t*>(dst + 8 * i) = pack_half2(o[4 * i + 2 * hr] * inv, o[4 * i + 2 * hr + 1] * inv);
+  }
 }
 
 // one CTA per sample: which 128-key blocks hold at least one valid key (blk_list / blk_count), and the invalid-key bit
@@ -505,22 +288,12 @@ __global__ void block_list_kernel(const uint8_t* __restrict__ key_mask, int L, i
       if (pos[i >> 2] >= 0) blk_words[((size_t)b * nkb + pos[i >> 2]) * 4 + (i & 3)] = wds[i];
 }
 
-template <int NT, int PM, int PT, int HW = 0>
-int launch_nt(cudaStream_t st, const CUtensorMap& tm, const AttnParams& p) {
-  using C = ACfg<NT>;
-  BG_TRY(ensure_dynamic_smem(reinterpret_cast<const void*>(&attn_kernel<NT, PM, PT, HW>), C::SMEM_BYTES));
-  const int nq = (p.L + 127) / 128;
-  dim3 grid((nq + NT - 1) / NT, NHEAD, p.B);
-  attn_kernel<NT, PM, PT, HW><<<grid, HW ? 512 : C::THREADS, C::SMEM_BYTES, st>>>(tm, p);
-  return check_launch("attn_kernel launch");
-}
-
 }  // namespace
 
 int launch_attention(cudaStream_t st, const AttnArgs& a) {
   BG_REQUIRE(a.qkv && a.out && a.B > 0 && a.L > 0, "attention: bad arguments");
   BG_REQUIRE(a.ldo % 8 == 0, "attention: output pitch must be a multiple of 8");
-  BG_REQUIRE(a.L <= 128 * ACfg<2>::MAX_KB, "attention: sequence longer than 8192 tokens is not supported");
+  BG_REQUIRE(a.L <= 128 * MAX_KB, "attention: sequence longer than 8192 tokens is not supported");
   BG_REQUIRE((a.blk_list == nullptr) == (a.blk_count == nullptr), "attention: blk_list and blk_count go together");
   CUtensorMap tm;
   BG_REQUIRE((a.seq_row0 == nullptr) == (a.seq_len == nullptr), "attention: seq_row0 and seq_len go together");
@@ -531,34 +304,11 @@ int launch_attention(cudaStream_t st, const AttnArgs& a) {
   p.key_mask = a.key_mask; p.blk_list = a.blk_list; p.blk_count = a.blk_count; p.blk_words = a.blk_words;
   p.seq_row0 = a.seq_row0; p.seq_len = a.seq_len;
   p.scale_log2 = 1.4426950408889634f / 8.0f;
-  static int poly = -1, ptmem = 1, pingpong = 1;   // environment knobs, read once per process
-  if (poly < 0) {
-    const char* e = getenv("BG_ATTN_POLY");   // exponentials on the FMA pipe: 0 | 1 (25 %, default) | 2 (50 %) | 3 (37.5 %)
-    poly = e ? atoi(e) : 1;
-    e = getenv("BG_ATTN_PT");                 // 0: P through shared memory (the round-1 path, kept as the A/B reference)
-    ptmem = e ? atoi(e) : 1;
-    e = getenv("BG_ATTN_PP");                 // XU token between the two softmax warpgroups
-    pingpong = e ? atoi(e) : 1;
-  }
-  p.pingpong = pingpong;
-  p.probe = 0;
-  if (a.L <= 128) return launch_nt<1, 0, 0>(st, tm, p);
-  if (ptmem) {
-    if (poly == 0) return launch_nt<2, 0x0000, 1, 1>(st, tm, p);
-    if (poly == 2) return launch_nt<2, 0xAAAA, 1, 1>(st, tm, p);
-    if (poly == 3) return launch_nt<2, 0xAA88, 1, 1>(st, tm, p);    // 37.5 %: 25 % in even, 50 % in odd 16-key groups
-    return launch_nt<2, 0x8888, 1, 1>(st, tm, p);
-  }
-  if (poly == 0) return launch_nt<2, 0x0000, 0, 1>(st, tm, p);
-  if (poly == 2) return launch_nt<2, 0xAAAA, 0, 1>(st, tm, p);
-  return launch_nt<2, 0x8888, 0, 1>(st, tm, p);
+  BG_TRY(ensure_dynamic_smem(reinterpret_cast<const void*>(&attn_kernel), SMEM_BYTES));
+  dim3 grid((a.L + BQ - 1) / BQ, NHEAD, a.B);
+  attn_kernel<<<grid, THREADS, SMEM_BYTES, st>>>(tm, p);
+  return check_launch("attn_kernel launch");
 }
-
-#ifdef BG_ATTN_TRACE
-extern "C" int bg_debug_attn_trace(long long* host_out) {
-  return check_cuda(cudaMemcpyFromSymbol(host_out, g_attn_trace, sizeof(long long) * 2 * 64 * 8), "trace copy");
-}
-#endif
 
 int launch_build_block_list(cudaStream_t st, const uint8_t* key_mask, int B, int L, int* blk_list, int* blk_count,
                             uint32_t* blk_words) {

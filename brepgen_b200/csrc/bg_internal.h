@@ -68,7 +68,7 @@ struct ConvGeom {
   int terms = 1;           // K = terms * taps * C: [A_hi W_hi (+ A_lo W_hi) + A_hi W_lo]
 };
 
-// ---- tcgen05 GEMM:  out[M,N] = epilogue( A[M,K] (fp16, pitch lda) * W[N,K]^T (fp16, pitch ldw) ) ----
+// ---- wgmma GEMM:  out[M,N] = epilogue( A[M,K] (fp16, pitch lda) * W[N,K]^T (fp16, pitch ldw) ) ----
 struct GemmEpilogue {
   void* out = nullptr;           // fp16 or fp32, pitch ldo (elements)
   int ldo = 0;
@@ -89,7 +89,7 @@ struct GemmEpilogue {
 int launch_gemm_f16(cudaStream_t st, const __half* A, int lda, const __half* W, int ldw, int M, int N, int K,
                     const GemmEpilogue& ep);
 
-// ---- tcgen05 flash attention over packed QKV [B*L, 2304] fp16 (q | k | v, head h at +64h) ----
+// ---- wgmma flash attention over packed QKV [B*L, 2304] fp16 (q | k | v, head h at +64h) ----
 struct AttnArgs {
   const __half* qkv = nullptr;      // [B*L, 3*768]
   __half* out = nullptr;            // [B*L, ldo] head h at column 64h

@@ -1,7 +1,7 @@
 // Greedy first-seen de-duplication of face / edge bounding boxes between cascade stages, on the device.
 //
 // Reference (host numpy loops with a D2H/H2D round trip per stage):
-//   surfaces  /root/reference/sample.py:159-183  np.round(bbox, 4); keep-list seeded with slot 0; slot i is a duplicate
+//   surfaces  sample.py:159-183  np.round(bbox, 4); keep-list seeded with slot 0; slot i is a duplicate
 //             iff for some kept k:  max|kept_k - bbox_i| < thr  OR  max|kept_k - reversed_corners(bbox_i)| < thr;
 //             survivors packed to the front, zero padded, mask True = padded.
 //   edges     sample.py:242-261  same test per VALID face over its E slots, no rounding, no packing: duplicates are

@@ -1,7 +1,7 @@
 // Denoiser handle: packs a reference checkpoint once, then runs a whole forward (embed -> 12 pre-norm encoder layers ->
 // final LayerNorm -> fc_out) as a fixed sequence of stream-ordered kernels.
 //
-// Mirrors /root/reference/network.py: SurfPosNet.forward :1107-1126, SurfZNet.forward :1176-1200,
+// Mirrors network.py: SurfPosNet.forward :1107-1126, SurfZNet.forward :1176-1200,
 // EdgePosNet.forward :1257-1286, EdgeZNet.forward :1357-1393; encoder = nn.TransformerEncoder(12 x
 // TransformerEncoderLayer(d=768, nhead=12, ff=1024, norm_first=True), LayerNorm) built at :1076-1078 etc.
 //

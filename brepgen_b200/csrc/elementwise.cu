@@ -2,7 +2,7 @@
 // MLPs, conditioning vectors, casts.  All HBM-bound: coalesced 16-byte accesses, one warp per token row.
 //
 // Reference: the Linear -> LayerNorm -> SiLU -> Linear embed MLPs and norm1/norm2/final norm of the encoder,
-// /root/reference/network.py:1080-1099 (and the analogous blocks of the other three nets); sincos_embedding :1043-1063.
+// network.py:1080-1099 (and the analogous blocks of the other three nets); sincos_embedding :1043-1063.
 #include <math.h>
 
 #include "bg_internal.h"

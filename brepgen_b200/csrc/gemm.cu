@@ -1,16 +1,16 @@
-// tcgen05 GEMM for sm_100a:  out[M,N] = epi( A[M,K] * W[N,K]^T ),  fp16 operands, fp32 accumulation in TMEM.
+// wgmma GEMM for sm_90a:  out[M,N] = epi( A[M,K] * W[N,K]^T ),  fp16 operands, fp32 accumulation in registers.
 //
 // This is the only dense linear contraction of the denoisers (reference: torch F.linear inside
-// nn.TransformerEncoderLayer / the embed MLPs, /root/reference/network.py:1076-1099) and of the VAE convs
-// (after im2col).  nn.Linear stores W as [N][K] row-major == K-major B operand, so weights are used as packed.
+// nn.TransformerEncoderLayer / the embed MLPs, network.py:1076-1099) and of the VAE convs (implicit GEMMs, ConvGeom).
+// nn.Linear stores W as [N][K] row-major == K-major B operand, so weights are used as packed.
 //
-// Structure (one persistent CTA per SM, 384 threads):
-//   warp 0  : TMA producer  (A tile 128x64, W tile BNx64, SWIZZLE_128B, STAGES-deep mbarrier ring)
-//   warp 1  : MMA issuer    (one elected thread: 4 x tcgen05.mma.kind::f16 M128 N=BN K16 per 64-wide k-block)
-//   warp 2  : TMEM allocator (2 x BN fp32 columns: accumulator double buffer -> epilogue overlaps next tile)
-//   warps 4-11: epilogue    (8 warps: TMEM lane quarter = warp % 4, column half = (warp - 4) / 4; tcgen05.ld 32x32b,
-//                            32x32 transpose through shared memory so that all global traffic is row-contiguous;
-//                            residual / row-vector loads issued BEFORE the TMEM wait so their latency overlaps it)
+// Structure (one persistent CTA per SM, 384 threads = 3 warpgroups, tile 128 x BN, BN = 128 or 256):
+//   warpgroup 0    : TMA producer (one elected thread: A tile 128x64, W tile BNx64, SWIZZLE_128B, STAGES-deep
+//                    mbarrier ring); gives its registers to the consumers (setmaxnreg)
+//   warpgroups 1-2 : consumers, one 64-row half of the tile each: 4 x wgmma m64nBNk16 per 64-wide k-block with both
+//                    operands read from shared memory, one k-block in flight while the previous stage is released;
+//                    the epilogue works straight from the accumulator registers while the producer already fills the
+//                    ring for the next tile
 // Roofline: tensor-bound; 2*M*N*K flop per launch.
 #include <stdlib.h>
 
@@ -19,8 +19,6 @@
 #include "ptx.cuh"
 
 namespace bg {
-
-int launch_gemm2_f16(cudaStream_t st, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p);   // gemm2.cu
 
 namespace {
 
@@ -33,12 +31,15 @@ struct Cfg {
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int TMEM_COLS = 2 * BN;
   static constexpr int BAR_BYTES = 256;
-  static constexpr int XPOSE_PITCH = GEMM_XPOSE_PITCH;
-  static constexpr int XPOSE_BYTES = 8 * 32 * XPOSE_PITCH * 4;            // one 32x32 fp32 staging tile per epilogue warp
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + XPOSE_BYTES + 1024;  // +1024: manual 1 KB alignment
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + 1024;  // +1024: manual 1 KB alignment
 };
+
+template <int BN>
+__device__ __forceinline__ void wgmma_tile_k16(float (&acc)[BN / 2], uint64_t a, uint64_t b, uint32_t accumulate) {
+  if constexpr (BN == 256) wgmma_m64n256k16_ss(acc, a, b, accumulate);
+  else wgmma_m64n128k16_ss(acc, a, b, accumulate);
+}
 
 template <int BN>
 __global__ void __launch_bounds__(384, 1)
@@ -49,41 +50,30 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
   uint64_t* empty = full + C::STAGES;
-  uint64_t* tfull = empty + C::STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
 
-  if (warp == 0 && elect_one()) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1 && elect_one()) {
     for (int i = 0; i < C::STAGES; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      mbar_init(&tempty[i], 256);
+      mbar_init(&empty[i], 256);     // every consumer thread releases the stage after its wgmma reads are complete
     }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc<C::TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int num_m = (p.M + BM - 1) / BM;
   const int num_n = p.N / BN;
   const int num_tiles = num_m * num_n;
   const int num_k = p.K / BK;
 
-  if (warp == 0) {
-    if (elect_one()) {
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -107,65 +97,38 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc = make_idesc_f16(BM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t accphase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tempty[acc], accphase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        const int nk = ((tile % num_n) * BN < p.n_short) ? p.k_short / BK : num_k;
-        for (int kb = 0; kb < nk; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + stage * C::STAGE_BYTES);
-          const uint32_t b_addr = a_addr + C::A_BYTES;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            umma_f16_ss(d_tmem, make_sw128_desc(a_addr + k * 32), make_sw128_desc(b_addr + k * 32), idesc,
-                        (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty[stage]);
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tfull[acc]);
-        acc ^= 1;
-        if (acc == 0) accphase ^= 1;
-      }
-    }
-  } else if (warp >= 4) {
-    // Epilogue.  tcgen05.ld hands each thread one accumulator ROW (32 consecutive columns per chunk); writing that
-    // straight out would make every global instruction touch 32 different rows.  Each warp therefore transposes its
-    // 32x32 chunk through a private shared-memory tile, after which lane == column: every residual / row-vector load and
-    // every store instruction covers one contiguous 128-byte (fp32) or 64-byte (fp16) row segment.
-    const int ew = (warp - 4) & 3;            // TMEM lane quarter this warp may access
-    const int half = (warp - 4) >> 2;         // column half of the tile
-    constexpr int CHUNKS = BN / 64;           // 32-column chunks per half
-    constexpr int PITCH = GEMM_XPOSE_PITCH;
-    float* xp = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE_BYTES + C::BAR_BYTES) + (warp - 4) * 32 * PITCH;
-    int acc = 0;
-    uint32_t accphase = 0;
+  } else {
+    setmaxnreg_inc<232>();
+    const int half = wg - 1;                  // rows [64 half, 64 half + 64) of the tile
+    float acc[BN / 2];
+    int stage = 0;
+    uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int m_blk = tile / num_n, n_blk = tile % num_n;
-      const int row0 = m_blk * BM + ew * 32;                 // first of this warp's 32 rows
-      const int colbase = n_blk * BN + half * (BN / 2);
-      mbar_wait(&tfull[acc], accphase);
-      tc_fence_after();
-      gemm_epilogue_tile<CHUNKS>(p, tmem_base + ((uint32_t)(ew * 32) << 16) + acc * BN + half * (BN / 2), row0, colbase, xp, lane);
-      tc_fence_before();
-      mbar_arrive(&tempty[acc]);
-      acc ^= 1;
-      if (acc == 0) accphase ^= 1;
+      const int nk = (n_blk * BN < p.n_short) ? p.k_short / BK : num_k;
+      int prev = -1;
+      for (int kb = 0; kb < nk; ++kb) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t a_addr = smem_u32(smem + stage * C::STAGE_BYTES) + half * 64 * 128;
+        const uint32_t b_addr = smem_u32(smem + stage * C::STAGE_BYTES + C::A_BYTES);
+        wgmma_fence_operand(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)
+          wgmma_tile_k16<BN>(acc, make_sw128_desc(a_addr + k * 32), make_sw128_desc(b_addr + k * 32), (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_fence_operand(acc);
+        wgmma_wait<1>();                      // the previous k-block's MMAs are done: release its stage
+        if (prev >= 0) mbar_arrive(&empty[prev]);
+        prev = stage;
+        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_operand(acc);
+      mbar_arrive(&empty[prev]);
+      gemm_epilogue_regs<BN>(p, acc, m_blk * BM + half * 64, n_blk * BN, warp & 3, lane);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc<C::TMEM_COLS>(tmem_base);
 }
 
 template <int BN>
@@ -193,24 +156,13 @@ int launch_gemm_f16(cudaStream_t st, const __half* A, int lda, const __half* W, 
   BG_REQUIRE(ep.resid == nullptr || (ep.ldr % 4 == 0 && !ep.out_f16 ? true : ep.ldr % 4 == 0), "gemm: resid pitch");
   BG_REQUIRE(ep.rowvec == nullptr || (ep.rows_per_vec > 0 && ep.ldv % 4 == 0), "gemm: rowvec");
   BG_REQUIRE(!ep.out_f16 || (ep.resid == nullptr && ep.rowvec == nullptr), "gemm: fp16 output supports bias / ReLU only");
-  static int two_cta = -1, small_m = -1;   // environment knobs, read once per process
-  if (two_cta < 0) {
-    const char* e = getenv("BG_GEMM_2CTA");   // 0: never use the CTA-pair kernel (gemm2.cu)
-    two_cta = e ? atoi(e) : 1;
-    e = getenv("BG_GEMM_SMALLM");             // 0: no small-problem tile selection
-    small_m = e ? atoi(e) : 1;
-  }
-  // Tile selection.  Large problems: 256 x 256 tiles on CTA pairs (half the weight traffic per CTA).  When that gives fewer
-  // tiles than there are CTA pairs (the surface stages: M = B x S of a few thousand rows), most SMs idle and the kernel time
-  // is the latency of ONE tile's serial main loop -- 128 x 128 tiles on single CTAs give 4x as many tiles with a 4x shorter
-  // main loop each.
+  // the epilogue reads bias and residual as column pairs (float2)
+  BG_REQUIRE((reinterpret_cast<uintptr_t>(ep.bias) & 7) == 0, "gemm: bias must be 8-byte aligned");
+  BG_REQUIRE((reinterpret_cast<uintptr_t>(ep.resid) & 7) == 0, "gemm: resid must be 8-byte aligned");
+  // Tile selection: 128 x 256 tiles halve the A traffic per flop; when they would leave SMs idle (the surface stages:
+  // M = B x S of a few thousand rows) 128 x 128 tiles give twice as many tiles with a main loop of half the length.
   int bn = (N % 256 == 0) ? 256 : 128;
-  // N % 256 != 0 (the Cout = 128 convolutions of the VAEs): 256 x 128 tiles on CTA pairs when there are enough of them
-  bool use2 = two_cta && (bn == 256 || (long long)((M + 255) / 256) * (N / 128) >= num_sms());
-  if (small_m && bn == 256 && (long long)((M + 255) / 256) * (N / 256) < num_sms() / 2) {
-    bn = 128;
-    use2 = false;
-  }
+  if (bn == 256 && (long long)((M + BM - 1) / BM) * (N / 256) < num_sms()) bn = 128;
   CUtensorMap tmA, tmB;
   const int a_cols = ep.a_kwrap > 0 ? ep.a_kwrap : K;
   BG_REQUIRE(ep.a_kwrap == 0 || (ep.a_kwrap % BK == 0 && ep.a_kwrap <= K), "gemm: a_kwrap must be a multiple of 64");
@@ -227,7 +179,7 @@ int launch_gemm_f16(cudaStream_t st, const __half* A, int lda, const __half* W, 
   } else {
     BG_TRY(make_tmap_2d_f16(&tmA, A, (uint64_t)M, (uint64_t)a_cols, (uint64_t)lda, BM));
   }
-  BG_TRY(make_tmap_2d_f16(&tmB, W, (uint64_t)N, (uint64_t)K, (uint64_t)ldw, use2 ? (uint32_t)bn / 2 : (uint32_t)bn));
+  BG_TRY(make_tmap_2d_f16(&tmB, W, (uint64_t)N, (uint64_t)K, (uint64_t)ldw, (uint32_t)bn));
   GemmParams p;
   p.M = M; p.N = N; p.K = K; p.a_kwrap = ep.a_kwrap; p.m_dev = ep.m_dev; p.row_map = ep.row_map;
   p.n_short = ep.n_short; p.k_short = ep.k_short;
@@ -239,7 +191,6 @@ int launch_gemm_f16(cudaStream_t st, const __half* A, int lda, const __half* W, 
   p.conv_taps = cg.taps; p.conv_kw = cg.kw; p.conv_cpb = cg.C / 64; p.conv_C = cg.C; p.conv_W = cg.W; p.conv_HW = cg.W * cg.H;
   p.conv_pad_w = cg.kw / 2; p.conv_pad_h = cg.taps > 0 ? (cg.taps / cg.kw) / 2 : 0;
   p.conv_lo_term = (cg.taps > 0 && cg.lo_plane && cg.terms == 3) ? 1 : -1;
-  if (use2) return launch_gemm2_f16(st, tmA, tmB, p);
   return bn == 256 ? launch_bn<256>(st, tmA, tmB, p) : launch_bn<128>(st, tmA, tmB, p);
 }
 

@@ -1,4 +1,4 @@
-// Epilogue shared by the 1-CTA (gemm.cu) and 2-CTA (gemm2.cu) tcgen05 GEMM kernels.
+// Parameters, implicit-convolution coordinates and register epilogue of the wgmma GEMM kernel (gemm.cu).
 #pragma once
 #include "bg_internal.h"
 #include "ptx.cuh"
@@ -44,97 +44,48 @@ __device__ __forceinline__ GemmParams gemm_resolve(const GemmParams& p) {
 }
 
 
-constexpr int GEMM_XPOSE_PITCH = 33;   // floats; +1 keeps both access patterns of the 32x32 staging tile conflict-free
-
-// One epilogue warp, one accumulator tile: `taddr` = TMEM address of column 0 of this warp's column half (lane quarter
-// already encoded), rows [row0, row0 + 32), columns [colbase, colbase + 32 * CHUNKS).  tcgen05.ld hands each thread one
-// accumulator ROW; fp32 outputs are transposed through the warp's private shared-memory tile `xp` so that every residual
-// / row-vector load and every store covers one contiguous 128-byte row segment; fp16 outputs (bias / ReLU only) are
-// written directly, 64 contiguous bytes per thread (the transpose would compete with the MMA operand reads for nothing).
-template <int CHUNKS>
-__device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, uint32_t taddr, int row0, int colbase, float* xp,
-                                                   int lane) {
-  constexpr int PITCH = GEMM_XPOSE_PITCH;
-#pragma unroll 1
-      for (int c = 0; c < CHUNKS; ++c) {
-        const int col0 = colbase + c * 32;
-        const int col = col0 + lane;
-        // additive terms in the transposed (lane == column) layout: issue the loads before touching TMEM
-        const float bias = p.bias ? __ldg(p.bias + col) : 0.f;
-        float add[32];
-        if (p.resid && !p.out_f16) {
+// One consumer warpgroup, one 64 x BN accumulator tile held in registers in the wgmma m64nBN fp32 layout: warp w of
+// the warpgroup owns rows 16w + lane / 4 (acc[4i], acc[4i + 1]) and 16w + 8 + lane / 4 (acc[4i + 2], acc[4i + 3]) at
+// columns 8i + 2 (lane % 4) + {0, 1}.  Each quad of lanes therefore covers 8 contiguous columns (32 B in fp32) of a row,
+// and the epilogue works on column pairs: float2 loads of bias / residual, float2 or half2 stores.
+template <int BN>
+__device__ __forceinline__ void gemm_epilogue_regs(const GemmParams& p, const float (&acc)[BN / 2], int row0, int col0,
+                                                   int warp_in_wg, int lane) {
 #pragma unroll
-          for (int rr = 0; rr < 32; ++rr) {
-            const int row = row0 + rr;
-            add[rr] = row < p.M ? p.resid[(size_t)row * p.ldr + col] : 0.f;
-          }
-        } else {
+  for (int hr = 0; hr < 2; ++hr) {
+    const int row = row0 + warp_in_wg * 16 + hr * 8 + (lane >> 2);
+    if (row >= p.M) continue;
+    const float* rv = (p.rowvec && !p.out_f16)
+                          ? p.rowvec + (size_t)((p.row_map ? p.row_map[row] : row) / p.rows_per_vec) * p.ldv : nullptr;
+    const float* rs = (p.resid && !p.out_f16) ? p.resid + (size_t)row * p.ldr : nullptr;
 #pragma unroll
-          for (int rr = 0; rr < 32; ++rr) add[rr] = 0.f;
-        }
-        if (p.rowvec && !p.out_f16) {
-#pragma unroll
-          for (int rr = 0; rr < 32; ++rr) {
-            const int row = row0 + rr;
-            if (row < p.M)
-              add[rr] += __ldg(p.rowvec + (size_t)((p.row_map ? p.row_map[row] : row) / p.rows_per_vec) * p.ldv + col);
-          }
-        }
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(taddr + c * 32, r);
-        tmem_ld_wait();
-        if (p.out_f16) {
-          // fp16 outputs (bias / ReLU only): 64 contiguous bytes per thread, written directly -- the shared-memory
-          // transpose would compete with the MMA operand reads (96 B/clk of the 128 B/clk smem bandwidth) for no gain
-          const int row = row0 + lane;
-          if (row < p.M) {
-            float v[32];
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-            if (p.bias) {
-              const float4* bp = reinterpret_cast<const float4*>(p.bias + col0);
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float4 t = __ldg(bp + i);
-                v[4 * i] += t.x; v[4 * i + 1] += t.y; v[4 * i + 2] += t.z; v[4 * i + 3] += t.w;
-              }
-            }
-            if (p.relu) {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i], 0.f);
-            }
-            uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<__half*>(p.out) + (size_t)row * p.ldo + col0);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              __half2 h0 = __floats2half2_rn(v[8 * i], v[8 * i + 1]);
-              __half2 h1 = __floats2half2_rn(v[8 * i + 2], v[8 * i + 3]);
-              __half2 h2 = __floats2half2_rn(v[8 * i + 4], v[8 * i + 5]);
-              __half2 h3 = __floats2half2_rn(v[8 * i + 6], v[8 * i + 7]);
-              uint4 u;
-              u.x = *reinterpret_cast<uint32_t*>(&h0);
-              u.y = *reinterpret_cast<uint32_t*>(&h1);
-              u.z = *reinterpret_cast<uint32_t*>(&h2);
-              u.w = *reinterpret_cast<uint32_t*>(&h3);
-              op[i] = u;
-            }
-          }
-          continue;
-        }
-        __syncwarp();                                        // previous chunk's reads of xp are done
-#pragma unroll
-        for (int i = 0; i < 32; ++i) xp[lane * PITCH + i] = __uint_as_float(r[i]);
-        __syncwarp();
-        {
-          float* ob = reinterpret_cast<float*>(p.out);
-#pragma unroll
-          for (int rr = 0; rr < 32; ++rr) {
-            float v = xp[rr * PITCH + lane] + bias + add[rr];
-            if (p.relu) v = fmaxf(v, 0.f);
-            const int row = row0 + rr;
-            if (row < p.M) ob[(size_t)row * p.ldo + col] = v;
-          }
-        }
+    for (int i = 0; i < BN / 8; ++i) {
+      const int col = col0 + 8 * i + 2 * (lane & 3);
+      float v0 = acc[4 * i + 2 * hr], v1 = acc[4 * i + 2 * hr + 1];
+      if (p.bias) {
+        const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+        v0 += b.x;
+        v1 += b.y;
       }
+      if (rv) {
+        v0 += __ldg(rv + col);
+        v1 += __ldg(rv + col + 1);
+      }
+      if (rs) {
+        const float2 r = *reinterpret_cast<const float2*>(rs + col);
+        v0 += r.x;
+        v1 += r.y;
+      }
+      if (p.relu) {
+        v0 = fmaxf(v0, 0.f);
+        v1 = fmaxf(v1, 0.f);
+      }
+      if (p.out_f16)
+        *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(p.out) + (size_t)row * p.ldo + col) = pack_half2(v0, v1);
+      else
+        *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + (size_t)row * p.ldo + col) = make_float2(v0, v1);
+    }
+  }
 }
 
 }  // namespace bg

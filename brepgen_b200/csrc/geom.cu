@@ -1,6 +1,6 @@
 // Post-decode geometry glue on the device (SURVEY.md 8(f) row 3): the O(n^2) numeric cores of the reference's per-CAD
 // post-processing between the VAE decoders and OpenCASCADE (construct_brep, out of scope):
-//   edge end points            /root/reference/sample.py:316-329   (+ utils.py:48-59 compute_bbox_center_and_size)
+//   edge end points            sample.py:316-329   (+ utils.py:48-59 compute_bbox_center_and_size)
 //   nearest "other" end point  utils.py:403-421 edge2loop, and the across-face centre search utils.py:505-524
 //   close-centre matrix        utils.py:556-561
 //   same-endpoints / z match   utils.py:607-619 detect_shared_edge

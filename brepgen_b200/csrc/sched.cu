@@ -1,7 +1,7 @@
 // Fused scheduler updates (HBM-bound elementwise): classifier-free-guidance combine + DDPM posterior step with
 // in-kernel Philox noise, and the PNDM transfer step with its Adams-Bashforth / Runge-Kutta combination of the eps
 // history.  Replaces ~15 scalar-broadcast torch launches per diffusers step (SURVEY.md Appendix A.3/A.4;
-// call sites /root/reference/sample.py:132-137,148-153,195-202,...).
+// call sites sample.py:132-137,148-153,195-202,...).
 // Algorithmic bytes per element: DDPM 4 (eps) [+4 uncond] + 4 (x) + 4 (out) [+4 explicit noise]; PNDM 4*(2 + #history).
 #include <math.h>
 

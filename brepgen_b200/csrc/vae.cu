@@ -1,11 +1,11 @@
 // Surface (2-D) and edge (1-D) VAE decoders: latents -> 32x32 / 32-point control grids.
 //
-// Reference: AutoencoderKLFastDecode.forward /root/reference/network.py:1013-1040 (diffusers 0.27 `Decoder`, cfg
+// Reference: AutoencoderKLFastDecode.forward network.py:1013-1040 (diffusers 0.27 `Decoder`, cfg
 // sample.py:72-82) and AutoencoderKL1DFastDecode.forward network.py:846-858 (Decoder1D :188-299, UNetMidBlock1D :51-83,
 // UpBlock1D :30-48, cfg sample.py:86-97); layer-by-layer arithmetic: SURVEY.md Appendix A.1 / A.2.
 //
 // Layout: activations are channels-last ([sample][position][channel]), fp32 for the residual stream and fp16 for GEMM
-// operands.  Convolutions are IMPLICIT GEMMs on the tcgen05 GEMM kernels (gemm.cu / gemm2.cu, ConvGeom): the A tile of
+// operands.  Convolutions are IMPLICIT GEMMs on the wgmma GEMM kernel (gemm.cu, ConvGeom): the A tile of
 // k-block (term, tap, 64-channel chunk) is a TMA box of the channels-last image shifted by the tap's offset, out-of-range
 // coordinates zero-filled = the padding, so the im2col matrix only ever exists as shared-memory tiles (round 1 / early
 // round 2 materialised it in HBM: ~9x the activation traffic and ~40 % of the decode time).  The few shapes a box cannot
@@ -28,11 +28,12 @@ inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
 inline int round64(int k) { return (k + 63) / 64 * 64; }
 
 // Number of product terms of the compensated GEMMs, fixed per handle at creation:
-//   3: A_hi W_hi + A_lo W_hi + A_hi W_lo   (activations AND weights split; 9.4e-5 / 3.6e-5 against the oracle)
+//   3: A_hi W_hi + A_lo W_hi + A_hi W_lo   (activations AND weights split)
 //   2: A_hi W_hi + A_hi W_lo               (weights split only: the systematic part of the fp16 error) -- 1/3 less GEMM work
 //                                           and no lo plane in the im2col matrices
-// Measured on B200 against the fp32 oracle (bar 1e-3): edge decoder 4.1-4.4e-4 with 2 terms -> default 2 (-27 % time);
-// surface decoder 1.3e-3 and the encoders 6.6-9e-4 with 2 terms -> they keep 3.  BREPGEN_B200_VAE_TERMS = 2 | 3 overrides.
+// Relative L2 errors against the fp32 oracle (bar 1e-3), measured on an H100 with 3 / 2 terms: surface decoder 9.4e-5 /
+// 1.3e-3, edge decoder 3.6e-5 / 4.1-4.3e-4, encoders <= 1.1e-4 / 6.4-9.0e-4.  So the edge decoder defaults to 2 terms (a
+// third less GEMM work); the surface decoder, over the bar with 2, and the encoders, close to it, keep 3.  BREPGEN_B200_VAE_TERMS = 2 | 3 overrides.
 int vae_terms_for(int kind) {
   const char* e = getenv("BREPGEN_B200_VAE_TERMS");
   if (e && (atoi(e) == 2 || atoi(e) == 3)) return atoi(e);

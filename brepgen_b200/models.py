@@ -7,7 +7,7 @@
 
 so `sample.py:56-70` (`Net(use_cf); load_state_dict(torch.load(p)); .to(device).eval()`) and every call in the six
 sampling loops work unchanged.  The parameters live in an nn.Module tree whose state_dict keys equal the
-reference's; the arithmetic runs in libbrepgen_b200.so (tcgen05 GEMM + flash attention, see csrc/).  Inference
+reference's; the arithmetic runs in libbrepgen_b200.so (wgmma GEMM + flash attention, see csrc/).  Inference
 only: there is no autograd and no CPU path -- calling forward on a CPU tensor or with is_train=True raises.
 Returned predictions are fp32 (the reference returns fp16 under its autocast context, sample.py:121).
 """
@@ -188,7 +188,7 @@ class _Denoiser(nn.Module):
             raise RuntimeError("brepgen_b200 denoisers are inference-only (is_train=True is the reference's training path)")
         self._check_shapes(x, surfPos, surfZ, edgePos, mask)
         if not x.is_cuda:
-            raise RuntimeError("brepgen_b200 has no CPU path: inputs must be CUDA tensors on an sm_100 device")
+            raise RuntimeError("brepgen_b200 has no CPU path: inputs must be CUDA tensors on an sm_90 (H100) device")
         dev = x.device
         with torch.cuda.device(dev):
             self._ensure_packed(dev)

@@ -1,6 +1,6 @@
 """Post-decode geometry glue with the reference's function surface (SURVEY.md 8(f) row 3).
 
-Drop-in for the per-CAD post-processing of /root/reference/sample.py:303-355 up to (not including) `construct_brep`:
+Drop-in for the per-CAD post-processing of sample.py:303-355 up to (not including) `construct_brep`:
 
     edge_endpoints(edge_pos_cad, edge_ncs_cad, edge_mask_cad)                    sample.py:316-329
     detect_shared_vertex(edgeV_cad, edge_mask_cad, edgeV_bbox)                   utils.py:463-586
@@ -15,7 +15,7 @@ same-end-points / latent-distance matrices, the closed-form edge fit, the surfac
 the 200-step AdamW fit of one translation per face against the one-directional Chamfer distance, which the reference runs as
 one chamferdist call per face and iteration and which here is ONE kernel launch for all faces and iterations.  What stays on
 the host is the bookkeeping over python lists and sets (loop closing, T-junction merging), a few dozen items per CAD.
-No CPU fallback: the library must be present and the device an sm_100 GPU.
+No CPU fallback: the library must be present and the device an sm_90 (H100) GPU.
 """
 from __future__ import annotations
 

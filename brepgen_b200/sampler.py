@@ -1,4 +1,4 @@
-"""The diffusion half of the reference's `sample()` (/root/reference/sample.py:120-299), device resident.
+"""The diffusion half of the reference's `sample()` (sample.py:120-299), device resident.
 
 Same stage order, tensor shapes, late face-count increase (sample.py:140-142), classifier-free guidance
 (sample.py:46-51,132-134), de-duplication semantics (sample.py:159-183, 242-261), final masking and latent -> grid

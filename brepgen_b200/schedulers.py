@@ -1,6 +1,6 @@
 """Drop-in DDPMScheduler / PNDMScheduler with the diffusers 0.27 interface used by the reference.
 
-Call sites mirrored (all in /root/reference): constructors sample.py:101-117 and trainer.py:285-292;
+Call sites mirrored (all in the reference): constructors sample.py:101-117 and trainer.py:285-292;
 `set_timesteps(n)` + `.timesteps[...]` slicing sample.py:128-129,144-145; `.step(pred, t, x).prev_sample`
 sample.py:137,153,202,222,236,282; `.add_noise(x, noise, t)` trainer.py:348; `.config.num_train_timesteps` trainer.py:330.
 

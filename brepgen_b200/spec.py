@@ -3,7 +3,7 @@
 These are the reference's checkpoint layouts, which are part of the drop-in boundary
 (SURVEY.md §8b): `sample.py:56-70` does `Net(use_cf).load_state_dict(torch.load(path))`.
 
-  denoisers : /root/reference/network.py:1066-1105 (SurfPosNet), :1129-1174 (SurfZNet),
+  denoisers : network.py:1066-1105 (SurfPosNet), :1129-1174 (SurfZNet),
               :1203-1255 (EdgePosNet), :1289-1355 (EdgeZNet); encoder = nn.TransformerEncoder
               (12 pre-norm layers d=768, 12 heads, FFN 1024) + final LayerNorm.
 """

@@ -6,7 +6,7 @@ Every tensor is drawn from its own generator seeded by crc32(key) + seed, so the
 not depend on module construction order or on which framework class holds the parameter.
 
 Magnitudes follow torch's default inits used by the reference
-(/root/reference/network.py:1066-1393 builds stock nn.Linear / nn.LayerNorm /
+(network.py:1066-1393 builds stock nn.Linear / nn.LayerNorm /
 nn.TransformerEncoderLayer): 2-D weights U(+-1/sqrt(fan_in)), LayerNorm/GroupNorm weights
 1 + 0.1 N(0,1) (non-trivial on purpose so the affine path is exercised), biases 0.05 N(0,1).
 """

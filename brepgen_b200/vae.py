@@ -85,7 +85,7 @@ class _VaeModule(nn.Module):
             raise RuntimeError(f"{type(self).__name__}: expected a non-empty {want_dim}-D tensor with 3 channels, "
                                f"got {tuple(z.shape)}")
         if not z.is_cuda:
-            raise RuntimeError("brepgen_b200 has no CPU path: z must be a CUDA tensor on an sm_100 device")
+            raise RuntimeError("brepgen_b200 has no CPU path: z must be a CUDA tensor on an sm_90 (H100) device")
         dev = z.device
         z = z.detach().float().contiguous()
         N = z.shape[0]

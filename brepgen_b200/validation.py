@@ -1,5 +1,5 @@
 """Forward-only validation of the four latent-diffusion trainers -- the reference's `test_val()` loop bodies
-(/root/reference/trainer.py:383-407 SurfPos, :570-603 SurfZ, :764-798 EdgePos, :987-1026 EdgeZ): frozen VAE encoders ->
+(trainer.py:383-407 SurfPos, :570-603 SurfZ, :764-798 EdgePos, :987-1026 EdgeZ): frozen VAE encoders ->
 latents, noise at the fixed timesteps {10, 50, 100[, 200, 500]} - 1, one denoiser forward per timestep, masked MSE of the
 noise prediction summed over the batch (the trainer divides the accumulated sums by the number of samples seen).
 

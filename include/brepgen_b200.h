@@ -1,4 +1,4 @@
-/* brepgen_b200 -- C ABI of the B200-native BrepGen sampling path (libbrepgen_b200.so).
+/* brepgen_b200 -- C ABI of the H100-native BrepGen sampling path (libbrepgen_b200.so).
  *
  * The reference (samxuxiang/BrepGen) is pure Python and has NO FFI of its own: its boundary for this path is the
  * Python class surface  SurfPosNet/SurfZNet/EdgePosNet/EdgeZNet.forward (network.py:1107,1176,1257,1357),
@@ -27,7 +27,7 @@ extern "C" {
 typedef enum {
   BG_STATUS_OK = 0,
   BG_STATUS_BAD_ARG = -1,
-  BG_STATUS_UNSUPPORTED_ARCH = -2,   /* not an sm_100 device */
+  BG_STATUS_UNSUPPORTED_ARCH = -2,   /* not an sm_90 (H100) device */
   BG_STATUS_CUDA = -3,
   BG_STATUS_WORKSPACE = -4,          /* workspace too small */
   BG_STATUS_MISSING_WEIGHT = -5
@@ -37,7 +37,7 @@ int bg_version(void);
 const char* bg_last_error(void);
 /* number of CUDA kernels this library has launched so far in this process (bench.py's gpu_launches) */
 uint64_t bg_launch_count(void);
-/* 0 if the current device is sm_100; BG_STATUS_UNSUPPORTED_ARCH otherwise */
+/* 0 if the current device is sm_90 (H100); BG_STATUS_UNSUPPORTED_ARCH otherwise */
 int bg_check_device(void);
 
 /* ---------------------------------------------------------------------------------------------------------------

@@ -1,4 +1,4 @@
-"""ORACLE (test infrastructure): CPU restatement of the cascade driver /root/reference/sample.py:120-299.
+"""ORACLE (test infrastructure): CPU restatement of the cascade driver sample.py:120-299.
 
 sample.py itself cannot be imported here (it imports OpenCASCADE at :9 and hard-codes .cuda() at :48,130,...), so the
 loop is restated device-agnostically around the oracle denoisers (oracle/denoisers.py, pinned to the reference's own

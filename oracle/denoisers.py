@@ -5,7 +5,7 @@ import this module; the product path (brepgen_b200/) never does.
 
 Restates, as plain functions over a state dict (no nn.Module, so nothing is shared with the
 reference's class structure):
-  sincos_embedding   /root/reference/network.py:1043-1063  (cos first, then sin; fp32)
+  sincos_embedding   network.py:1043-1063  (cos first, then sin; fp32)
   embed MLPs         network.py:1080-1099 etc.  Linear -> LayerNorm(eps 1e-5) -> SiLU -> Linear
   encoder            network.py:1076-1078 = torch nn.TransformerEncoder(12 x pre-norm layer, final LN):
                      x += out_proj(softmax(q k^T / 8 + kpm) v);  x += W2 relu(W1 LN2(x) + b1) + b2
@@ -15,7 +15,7 @@ reference's class structure):
   EdgeZNet.forward   network.py:1357-1393   (token = 12 edge latent + 6 vertex coords)
 
 Pinned: tests/golden/denoisers_*.npz hold outputs of the reference's OWN classes (imported from
-/root/reference with `diffusers` stubbed, see tests/golden/make_golden.py) on the same synthetic
+the reference with `diffusers` stubbed, see tests/golden/make_golden.py) on the same synthetic
 weights; tests/test_oracle_golden.py checks this restatement against them.
 """
 from __future__ import annotations

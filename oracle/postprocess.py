@@ -4,7 +4,7 @@ VAE decoders and OpenCASCADE -- SURVEY.md 8(f) row 3.
 Only tests/ and tests/golden/make_golden_post.py import this module; brepgen_b200/ never does.
 
 Restated (numpy, statement order of the reference so that vertex / edge numbering comes out identical):
-  edge_endpoints          /root/reference/sample.py:316-329  (+ utils.py:48-59 compute_bbox_center_and_size)
+  edge_endpoints          sample.py:316-329  (+ utils.py:48-59 compute_bbox_center_and_size)
   edge2loop               utils.py:403-421
   keep_largelist          utils.py:424-460
   detect_shared_vertex    utils.py:463-586
@@ -12,7 +12,7 @@ Restated (numpy, statement order of the reference so that vertex / edge numberin
   joint_optimize          utils.py:672-776 (torch CPU; `chamfer_reverse_sum` stands in for chamferdist.ChamferDistance)
 
 Pinned: tests/golden/post_golden.npz holds the outputs of the reference's OWN function texts, exec()'d from
-/root/reference/utils.py and sample.py by tests/golden/make_golden_post.py on synthetic closed B-reps;
+utils.py and sample.py by tests/golden/make_golden_post.py on synthetic closed B-reps;
 tests/test_oracle_post.py checks this restatement against them (ids exact, coordinates to fp32 round-off).
 PARITY UNPINNED for one dependency: `chamferdist` (requirements.txt, absent offline).  Its published semantics are
 restated here -- ChamferDistance()(source, target, bidirectional=False, reverse=True) = sum over TARGET points of the

@@ -9,10 +9,11 @@ The reference (samxuxiang/BrepGen) is a script collection without packaging, and
 `diffusers` names it imports; its denoiser classes then run their stock code path (nn.TransformerEncoder etc.).
 
 Where the file comes from:
-  * /root/reference/network.py in the build container;
-  * baseline/_ref/network.py on the GPU box: `install_reference()` (called by __graft_entry__.build() whenever
-    /root/reference is present) places an unmodified copy there.  baseline/_ref/ is git-ignored (the reference's source
-    never enters this repository's history) but not gpurun-ignored, so it travels with the snapshot like the built .so.
+  * the reference checkout named by $BREPGEN_REFERENCE (default /root/reference),
+    when it is readable;
+  * oracle/_ref/network.py: `install_reference()` (called by __graft_entry__.build() whenever the reference checkout is
+    readable) places an unmodified copy there, so that a copy of the built tree carries it to machines without the
+    checkout.  oracle/_ref/ is git-ignored: the reference's source never enters this repository's history.
 """
 from __future__ import annotations
 
@@ -24,14 +25,14 @@ import types
 from typing import Optional
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_SRC = "/root/reference"
-REF_INSTALL = os.path.join(ROOT, "baseline", "_ref")
+REF_SRC = os.environ.get("BREPGEN_REFERENCE", "/root/reference")
+REF_INSTALL = os.path.join(ROOT, "oracle", "_ref")
 _FILES = ("network.py",)            # the only reference module the denoiser path needs
 
 
 def install_reference() -> Optional[str]:
-    """copy the reference module(s) of this path, unmodified, into baseline/_ref/ (no-op without /root/reference)"""
-    if not os.path.isdir(REF_SRC):
+    """copy the reference module(s) of this path, unmodified, into oracle/_ref/ (no-op without a readable checkout)"""
+    if not REF_SRC or not all(os.access(os.path.join(REF_SRC, f), os.R_OK) for f in _FILES):
         return REF_INSTALL if os.path.exists(os.path.join(REF_INSTALL, _FILES[0])) else None
     os.makedirs(REF_INSTALL, exist_ok=True)
     for f in _FILES:
@@ -41,7 +42,7 @@ def install_reference() -> Optional[str]:
 
 def reference_dir() -> Optional[str]:
     for d in (REF_SRC, REF_INSTALL):
-        if os.path.exists(os.path.join(d, _FILES[0])):
+        if d and os.access(os.path.join(d, _FILES[0]), os.R_OK):
             return d
     return None
 
@@ -90,8 +91,8 @@ def load_reference_network(required: bool = True):
     d = reference_dir()
     if d is None:
         if required:
-            raise RuntimeError("reference network.py not found (neither /root/reference nor baseline/_ref): "
-                               "run __graft_entry__.build() in the build container")
+            raise RuntimeError("reference network.py not found (neither $BREPGEN_REFERENCE nor oracle/_ref): "
+                               "run __graft_entry__.build() where the reference checkout is readable")
         return None
     _stub_diffusers()
     spec = importlib.util.spec_from_file_location("brepgen_reference_network", os.path.join(d, "network.py"))

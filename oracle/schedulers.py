@@ -1,6 +1,6 @@
 """ORACLE (test infrastructure): CPU restatement of diffusers 0.27 DDPMScheduler / PNDMScheduler arithmetic.
 
-diffusers==0.27 (requirements.txt:5 of the reference) is a third-party dependency that is absent from /root/reference and
+diffusers==0.27 (requirements.txt:5 of the reference) is a third-party dependency that is absent from the reference and
 from this image, so its code cannot be executed here and the reference itself holds no golden vector for it.
 PINNED by the known answers of diffusers' own scheduler tests (tests/test_oracle_sched_kat.py): the full 1000-step DDPM
 loop with injected noise (|x| sum 258.9606) and the PRK + PLMS loops of PNDM (198.1318; beta_start = 0.01: 186.9482) over the

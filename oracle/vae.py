@@ -9,10 +9,10 @@ decimals, and the block wiring (resnet -> upsample; resnet -> attention -> resne
 Downsample2DBlockTests.test_downsample_with_conv / DownEncoderBlock2DTests (with diffusers' default symmetric padding; the
 asymmetric padding=0 variant the VAE uses differs by the one F.pad line).  1-D leaves (ResConvBlock, SelfAttention1d, Upsample1d / Downsample1d; diffusers has no known-answer test for them)
 remain PARITY UNPINNED.  The arithmetic lives in diffusers==0.27 (requirements.txt:5 of the reference), which is absent from
-/root/reference and from this image: `Decoder`, `UNetMidBlock2D`, `UpDecoderBlock2D`, `ResnetBlock2D`, `Attention`,
+the reference and from this environment: `Decoder`, `UNetMidBlock2D`, `UpDecoderBlock2D`, `ResnetBlock2D`, `Attention`,
 `Upsample2D` (surface) and `ResConvBlock`, `SelfAttention1d`, `Upsample1d` (edge).  This file restates their published
 structure (SURVEY.md Appendix A.1 / A.2) around the reference's own wrappers
-    AutoencoderKLFastDecode.forward      /root/reference/network.py:1013-1040   (cfg sample.py:72-82)
+    AutoencoderKLFastDecode.forward      network.py:1013-1040   (cfg sample.py:72-82)
     AutoencoderKL1DFastDecode.forward    network.py:846-858, Decoder1D :188-299, UNetMidBlock1D :51-83, UpBlock1D :30-48
                                          (cfg sample.py:86-97)
 and is anchored on: input/output shapes consumed at sample.py:289-294, the state-dict key sets and the parameter counts

@@ -10,7 +10,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (sm_90a)")
 
 
 def pytest_collection_modifyitems(config, items):

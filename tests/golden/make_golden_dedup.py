@@ -2,7 +2,7 @@
 
     python tests/golden/make_golden_dedup.py        # writes tests/golden/dedup_golden.npz
 
-/root/reference/sample.py cannot be imported (OpenCASCADE, hard-coded .cuda()), but its de-duplication code is plain
+sample.py cannot be imported (OpenCASCADE, hard-coded .cuda()), but its de-duplication code is plain
 numpy / torch: this script reads the statements at sample.py:159-183 (surfaces) and :242-261 (edges) from the reference
 file at generation time, dedents them and exec()s them verbatim on seeded inputs, with `Tensor.cuda` patched to the
 identity.  Nothing of the reference is copied into the repository; the committed .npz holds inputs and outputs only.
@@ -15,7 +15,7 @@ import textwrap
 import numpy as np
 import torch
 
-REF = "/root/reference/sample.py"
+REF = os.path.join(os.environ.get("BREPGEN_REFERENCE", "/root/reference"), "sample.py")
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 THR = 0.08     # bbox_threshold of every mode in eval_config.yaml
 

@@ -2,7 +2,7 @@
 
     python tests/golden/make_golden_driver.py       # writes tests/golden/driver_golden.npz   (build container only)
 
-/root/reference/sample.py cannot be imported or run (OpenCASCADE import, checkpoints, hard-coded .cuda()), but the body of
+sample.py cannot be imported or run (OpenCASCADE import, checkpoints, hard-coded .cuda()), but the body of
 its sampling block -- sample.py:122-299: the six step loops, classifier-free batching and combine, the late increase, both
 de-duplications, the zeroing of removed edges and the decoder input preparation -- is plain torch / numpy.  This script
 reads those lines from the reference file at generation time, dedents them and exec()s them VERBATIM in a namespace where
@@ -27,7 +27,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
-REF = "/root/reference/sample.py"
+REF = os.path.join(os.environ.get("BREPGEN_REFERENCE", "/root/reference"), "sample.py")
 CASES = {  # name: (use_cf, batch, num_surfaces (before the late increase), num_edges, seed)
     "abc_like": (False, 2, 3, 3, 11),
     "furniture_like": (True, 2, 5, 4, 12),

@@ -3,9 +3,9 @@
     python tests/golden/make_golden_l4000.py        # writes tests/golden/denoisers_l4000_golden.npz
 
 BASELINE.json configs[2] runs the edge stages at S = 100 faces x E = 40 edges = ONE sequence of L = 4000 tokens per sample
-(/root/reference/network.py:1257-1286, 1357-1393).  The small goldens of make_golden.py (L = 5 / 15) only reach the
+(network.py:1257-1286, 1357-1393).  The small goldens of make_golden.py (L = 5 / 15) only reach the
 single-key-block attention path; these cases pin the exact kernel instantiation the headline number is measured on
-(2-tile flash attention over 32 key blocks, block lists with fully padded 128-key blocks, ragged masks, B >= 2 so the
+(flash attention over 32 key blocks, block lists with fully padded 128-key blocks, ragged masks, B >= 2 so the
 per-sample batch pitch of every buffer is exercised):
 
   edgepos_dense_b2      EdgePosNet, cf off, B = 2, nothing masked, scalar timestep

@@ -2,7 +2,7 @@
 
     python tests/golden/make_golden_post.py          # writes tests/golden/post_golden.npz
 
-/root/reference/utils.py cannot be imported (OpenCASCADE / chamferdist at module import).  The functions of this path are
+utils.py cannot be imported (OpenCASCADE / chamferdist at module import).  The functions of this path are
 plain numpy / torch, so their source text is cut out of the file with `ast` and exec()'d VERBATIM:
     compute_bbox_center_and_size  utils.py:48-59      edge2loop             utils.py:403-421
     keep_largelist                utils.py:424-460    detect_shared_vertex  utils.py:463-586
@@ -24,7 +24,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
-REF = "/root/reference"
+REF = os.environ.get("BREPGEN_REFERENCE", "/root/reference")
 CASES = {"box_a": (1, 8, 6), "box_b": (2, 7, 5), "box_c": (3, 10, 8)}       # seed, padded face slots, padded edge slots
 Z_THRESHOLD = 0.2                                                          # eval_config.yaml:10
 

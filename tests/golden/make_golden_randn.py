@@ -2,7 +2,7 @@
 
     python tests/golden/make_golden_randn.py        # writes tests/golden/randn_golden.npz   (build container only)
 
-/root/reference/utils.py cannot be imported (OpenCASCADE / chamferdist at its top), so the definition of `randn_tensor`
+utils.py cannot be imported (OpenCASCADE / chamferdist at its top), so the definition of `randn_tensor`
 (utils.py:60-97) is read from the reference file and exec()ed verbatim.  sample.py calls it as randn_tensor(shape) --
 no generator, no device -- i.e. the CPU global generator, fp32, then `.to(device)`; the four initial-noise draws of one
 cascade happen in the order surfPos, surfZ, edgePos, edgeZV (sample.py:126,189,208,267; the DDPM step noise in between
@@ -23,7 +23,7 @@ SHAPES = {"surfPos": (B, S0, 6), "surfZ": (B, S, 48), "edgePos": (B, S, E, 6), "
 
 
 def main():
-    lines = open("/root/reference/utils.py").read().splitlines()[60 - 1:97]
+    lines = open(os.path.join(os.environ.get("BREPGEN_REFERENCE", "/root/reference"), "utils.py")).read().splitlines()[60 - 1:97]
     ns = dict(torch=torch, Union=Union, Tuple=Tuple, List=List, Optional=Optional)
     exec(textwrap.dedent("\n".join(lines)), ns)
     torch.manual_seed(SEED)

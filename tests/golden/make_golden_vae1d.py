@@ -3,7 +3,7 @@
     python tests/golden/make_golden_vae1d.py        # writes tests/golden/vae1d_golden.npz   (build container only)
 
 AutoencoderKL1DFastDecode, Decoder1D, UNetMidBlock1D and UpBlock1D are defined by the reference itself
-(/root/reference/network.py:786-858, :188-299, :51-83, :30-48); only three leaf modules come from diffusers 0.27
+(network.py:786-858, :188-299, :51-83, :30-48); only three leaf modules come from diffusers 0.27
 (ResConvBlock, SelfAttention1d, Upsample1d -- absent here, no network).  This script imports the REAL network.py with those
 three leaves replaced by the nn.Module forms below (written from the published diffusers 0.27 `unet_1d_blocks.py`
 semantics, the same restatement oracle/vae.py uses in functional form), instantiates the reference's

@@ -2,7 +2,7 @@
 
     python tests/golden/make_golden_val.py        # writes tests/golden/val_golden.npz   (build container only)
 
-/root/reference/trainer.py cannot be imported (wandb, diffusers), but the bodies of its four `test_val()` loops --
+trainer.py cannot be imported (wandb, diffusers), but the bodies of its four `test_val()` loops --
 trainer.py:395-403, :579-596, :774-791, :997-1019: frozen-encoder latent pass, fixed-timestep noising, one forward, masked
 MSE -- are plain torch.  This script reads those lines from the reference file at generation time, dedents them and exec()s
 them VERBATIM in a namespace where `self.model` is the oracle denoiser (oracle/denoisers.py, itself pinned to the reference's
@@ -29,7 +29,7 @@ from oracle import denoisers as O                                               
 from oracle import vae as V                                                            # noqa: E402
 from oracle.schedulers import DDPMOracle                                               # noqa: E402
 
-REF = "/root/reference/trainer.py"
+REF = os.path.join(os.environ.get("BREPGEN_REFERENCE", "/root/reference"), "trainer.py")
 BLOCKS = {"surfpos": (395, 403), "surfz": (579, 596), "edgepos": (774, 791), "edgez": (997, 1019)}
 SEEDS = {"surfpos": 101, "surfz": 102, "edgepos": 103, "edgez": 104}
 B, S, E = 2, 4, 3

@@ -1,6 +1,6 @@
 """GPU: the CUDA-graph form of a DDPM loop (sampler.Cascade._loop_graph: step counter / timestep advance -> forward -> fused
 table-driven scheduler step, captured once and replayed) against the eager loop with the same Philox stream, and the whole
-cascade with graphs on vs off.  Loop body mirrored: /root/reference/sample.py:145-153; SURVEY.md 7.2 step 4."""
+cascade with graphs on vs off.  Loop body mirrored: sample.py:145-153; SURVEY.md 7.2 step 4."""
 import pytest
 import torch
 

@@ -1,10 +1,10 @@
 """GPU parity AT THE BENCHMARK'S OWN SHAPES (BASELINE.json configs[2]: S = 100 faces x E = 40 edges = L = 4000 tokens).
 
-Goldens = outputs of the reference's OWN EdgePosNet / EdgeZNet classes (/root/reference/network.py:1257-1286, 1357-1393)
+Goldens = outputs of the reference's OWN EdgePosNet / EdgeZNet classes (network.py:1257-1286, 1357-1393)
 at that shape, written by tests/golden/make_golden_l4000.py: B = 2 and 3, dense and ragged masks (whole 128-key blocks
 padded, 30 % random edge masks), scalar and per-sample timesteps, classifier-free labels on / off, plus a 4-step DDPM chain
-with injected noise.  This is the kernel instantiation the headline number is measured on (2-tile flash attention over 32
-key blocks with a block list, 2-CTA GEMMs at M = B * 4000, the multi-GB workspace carve).  Compared on valid tokens
+with injected noise.  This is the kernel instantiation the headline number is measured on (flash attention over 32 key blocks
+with a block list, one 128-row query tile per CTA, persistent GEMMs at M = B * 4000, the multi-GB workspace carve).  Compared on valid tokens
 (padded tokens are discarded by the cascade, sample.py:245,284); bar 1e-3 relative L2 (BASELINE.json).
 """
 import os

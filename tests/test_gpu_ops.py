@@ -42,9 +42,9 @@ GEMM_CASES = [
     (200, 128, 192, 0, 0, True, False, 7),
     (70, 768, 1536, 0, 0, True, False, 7),
     (384, 768, 2304, 0, 0, True, False, 3),
-    (128 * 170, 2304, 768, 1, 0, True, False, 0),   # 1530 tiles > 148 CTAs: ring + accumulator phases wrap
+    (128 * 170, 2304, 768, 1, 0, True, False, 0),   # 1530 tiles > 132 CTAs: ring phases wrap across tiles
     (128 * 170 + 5, 768, 1024, 0, 0, True, True, 0),
-    # N % 256 != 0 with many tiles: the CTA-pair kernel with 256 x 128 tiles (all three epilogues)
+    # N % 256 != 0 with many tiles: 128 x 128 tiles, persistent CTAs wrap (all three epilogues)
     (128 * 300, 128, 1152, 0, 0, True, False, 0),
     (128 * 300 + 7, 128, 576, 0, 0, True, True, 0),
     (128 * 300, 384, 256, 1, 1, True, False, 0),
@@ -83,6 +83,21 @@ def test_gemm(M, N, K, out_f16, relu, use_bias, use_resid, rpv):
     print(f"gemm M={M} N={N} K={K} f16={out_f16} rel_l2={err:.3e}")
     assert torch.isfinite(out.float()).all()
     assert err < (1e-3 if out_f16 else 2e-6), err
+
+
+def test_gemm_rejects_misaligned_epilogue_pointers():
+    """the epilogue reads bias and residual as float2 pairs: a pointer that is not 8-byte aligned is a bad argument
+    (status -1), caught before any launch"""
+    f = _ffi()
+    A = torch.zeros(128, 64, device="cuda", dtype=torch.float16)
+    W = torch.zeros(128, 64, device="cuda", dtype=torch.float16)
+    out = torch.zeros(128, 128, device="cuda")
+    buf = torch.zeros(128 * 128 + 2, device="cuda")
+    odd = buf.data_ptr() + 4
+    for bias, resid in ((odd, None), (None, odd)):
+        st = f.lib().bg_op_gemm_f16(A.data_ptr(), 64, W.data_ptr(), 64, 128, 128, 64, out.data_ptr(), 128, 0, 0, bias,
+                                    resid, 128, None, 1, 128, f.current_stream())
+        assert st == -1 and b"8-byte aligned" in f.lib().bg_last_error()
 
 
 def _attn_ref(qkv, B, L, mask):

@@ -2,7 +2,7 @@
 batch 64 (SURVEY.md section 8(d) input 2): single forwards at t in {999, 500, 249, 10, 0} and two 10-step chains
 (t = 999..990 and t = 9..0) with the step noise shared with the CPU fp32 oracle; bar 1e-3 relative (L2).
 
-Strict since round 2 (passed on the driver's B200 at the end of round 1).
+Strict: no expected failures.
 """
 import pytest
 import torch

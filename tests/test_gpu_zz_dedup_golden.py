@@ -1,7 +1,7 @@
 """GPU: the de-duplication kernels against the outputs of the reference's OWN statements (tests/golden/dedup_golden.npz,
 written by tests/golden/make_golden_dedup.py from sample.py:159-183 and :242-261): packed boxes and masks bit-exact.
 
-Strict since round 2 (passed on the driver's B200 at the end of round 1)."""
+Strict: no expected failures."""
 import os
 
 import numpy as np

@@ -4,7 +4,7 @@ block, sample.py:122-299, executed verbatim around stand-in networks (tests/gold
 tests/golden/make_golden_driver.py).  The same stand-ins (plain torch functions with the reference's forward signatures)
 are plugged into Cascade here, so everything between the network calls is the code under test.
 
-Strict since round 2 (passed on the driver's B200 at the end of round 1).
+Strict: no expected failures.
 """
 import os
 import sys

@@ -169,7 +169,7 @@ def test_shard_batch_partitions():
 
 
 def test_reference_arm_prints_contract_json():
-    """`bench.py --impl reference` (the reference's own classes on the host cores when baseline/_ref or /root/reference
+    """`bench.py --impl reference` (the reference's own classes on the host cores when oracle/_ref or $BREPGEN_REFERENCE
     holds network.py, else the oracle port) must print ONE JSON line with the contract keys."""
     import json
     import subprocess
@@ -228,7 +228,7 @@ def test_valid_token_flops_reduce_to_dense_when_nothing_is_masked():
 def test_reference_loader_runs_the_reference_classes_when_available():
     from oracle.reference_loader import load_reference_network, reference_dir
     if reference_dir() is None:
-        pytest.skip("neither /root/reference nor baseline/_ref present")
+        pytest.skip("neither $BREPGEN_REFERENCE nor oracle/_ref present")
     net = load_reference_network()
     m = net.SurfPosNet(False).eval()
     with torch.no_grad():

@@ -1,7 +1,7 @@
 """Oracle (oracle/denoisers.py) vs golden vectors produced by the reference's own classes.
 
 The fixtures in tests/golden/denoisers_golden.npz were written by tests/golden/make_golden.py, which
-imports /root/reference/network.py (diffusers stubbed) and runs SurfPosNet/SurfZNet/EdgePosNet/EdgeZNet
+imports network.py (diffusers stubbed) and runs SurfPosNet/SurfZNet/EdgePosNet/EdgeZNet
 (network.py:1066-1393) on synthetic weights.  Tolerance: fp32 re-association only (1e-5 of max|ref|).
 """
 import os

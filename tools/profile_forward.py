@@ -1,7 +1,6 @@
-"""Run a few forwards of one denoiser at ABC-eval shapes (for ncu launch lists / full captures).
+"""Run a few forwards of one denoiser at ABC-eval shapes (under a profiler of your choice).
 
-    ncu --metrics gpu__time_duration.sum --clock-control none --csv --log-file gpurun_out/launches.csv \
-        python tools/profile_forward.py --kind edgepos --batch 8 --iters 1
+    python tools/profile_forward.py --kind edgepos --batch 8 --iters 1
 """
 import argparse
 import os

@@ -22,11 +22,11 @@ def run(name, fn, *a):
 
 import test_gpu_ops as T   # noqa: E402
 run("gemm", T.test_gemm, 128, 256, 64, 0, 0, False, False, 0)
-run("gemm", T.test_gemm, 300, 768, 768, 0, 0, True, False, 0)          # 2-CTA kernel? small-M path: 128-wide tiles
+run("gemm", T.test_gemm, 300, 768, 768, 0, 0, True, False, 0)          # small-M path: 128-wide tiles
 run("gemm", T.test_gemm, 257, 1024, 768, 1, 1, True, False, 0)
 run("gemm", T.test_gemm, 513, 768, 1024, 0, 0, True, True, 0)
 run("gemm", T.test_gemm, 200, 128, 192, 0, 0, True, False, 7)
-run("gemm", T.test_gemm, 128 * 170, 2304, 768, 1, 0, True, False, 0)   # CTA-pair kernel, fp16 TMA-store epilogue
+run("gemm", T.test_gemm, 128 * 170, 2304, 768, 1, 0, True, False, 0)   # persistent tiles wrap, fp16 epilogue
 run("attention", T.test_attention, 2, 30, None, 0)
 run("attention", T.test_attention, 3, 100, "rand", 1)
 run("attention", T.test_attention, 1, 300, None, 0)
@@ -35,7 +35,7 @@ run("attention", T.test_attention, 2, 1000, "blocks", 1)
 run("layernorm", T.test_layernorm, 77, 0)
 run("scheduler steps", T.test_ddpm_and_pndm_step_kernels)
 if what != "ops-no-res1":
-    run("gemm", T.test_gemm, 128 * 170 + 5, 768, 1024, 0, 0, True, True, 0)   # CTA-pair kernel, TMA-staged residual epilogue
+    run("gemm", T.test_gemm, 128 * 170 + 5, 768, 1024, 0, 0, True, True, 0)   # persistent tiles wrap, residual epilogue
 if what == "all":
     import test_gpu_cascade as C
     import test_gpu_compaction as K
