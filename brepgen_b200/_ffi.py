@@ -87,6 +87,18 @@ def ptr(t) -> Optional[int]:
     return None if t is None else t.data_ptr()
 
 
+def named_tensors(state_dict, device):
+    """a state dict as the BgNamedTensor array bg_denoiser_create / bg_vae_create read (the array refers to the tensors'
+    memory: keep them alive until the call's stream has been synchronised)"""
+    import torch
+    arr = (BgNamedTensor * len(state_dict))()
+    for i, (k, v) in enumerate(state_dict.items()):
+        if v.device != device or v.dtype != torch.float32 or not v.is_contiguous():
+            raise RuntimeError(f"parameter {k} must be contiguous fp32 on {device} (call .to(device) first)")
+        arr[i].name, arr[i].data, arr[i].numel = k.encode(), v.data_ptr(), v.numel()
+    return arr
+
+
 def current_stream() -> int:
     import torch
     return torch.cuda.current_stream().cuda_stream

@@ -6,7 +6,11 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <functional>
+#include <map>
 #include <string>
+
+#include "../../include/brepgen_b200.h"
 
 namespace bg {
 
@@ -41,6 +45,37 @@ unsigned long long launch_count();
 int num_sms();   // of the current device (cached per device)
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) once per (kernel, device)
 int ensure_dynamic_smem(const void* func, int bytes);
+
+inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
+
+// Start of the caller's workspace rounded up to 1 KB (the bg_*_workspace_bytes sizes include that slack) in *base;
+// BG_ERR_WORKSPACE when `need` bytes from there do not fit in `bytes`.
+int align_workspace(void* ws, size_t bytes, size_t need, const char* what, char** base);
+
+// ---- weight packing: named fp32 device tensors in, one device arena out ----
+// A pack function runs twice over the same Packer: a dry pass (take() returns null, nothing is read) that only sizes the
+// arena, then a pass that fills it.  The first error is kept in `err` (and bg_last_error).
+struct Packer {
+  std::map<std::string, const BgNamedTensor*> by_name;
+  char* base = nullptr;
+  size_t off = 0;
+  bool dry = true;
+  cudaStream_t st = nullptr;
+  int err = 0;
+
+  Packer(const BgNamedTensor* weights, int n, void* stream);
+  const float* find(const std::string& name, int64_t numel);   // null (and err set) when missing or of the wrong size
+  template <class T>
+  T* take(size_t n) {
+    T* p = dry ? nullptr : reinterpret_cast<T*>(base + off);
+    off += align_up(n * sizeof(T));
+    return p;
+  }
+  float* copy_f32(const std::string& name, int64_t numel);
+  float* zeros(int64_t numel);
+};
+// pass 1 (size), cudaMalloc of *arena, pass 2 (fill); on error the arena is freed and *arena is null
+int pack_arena(Packer& pk, const std::function<int()>& pack, char** arena, size_t* arena_bytes);
 
 // ---- TMA descriptor creation (driver entry point resolved at run time; no link dependency on libcuda) ----
 // 2-D fp16 row-major [rows][cols] with row pitch ld (elements); box = {box_cols(=64), box_rows}; SWIZZLE_128B.

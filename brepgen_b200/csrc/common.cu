@@ -55,6 +55,66 @@ int ensure_dynamic_smem(const void* func, int bytes) {
   return BG_OK;
 }
 
+int align_workspace(void* ws, size_t bytes, size_t need, const char* what, char** base) {
+  *base = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(ws) + 1023) & ~uintptr_t(1023));
+  if (need + (size_t)(*base - reinterpret_cast<char*>(ws)) > bytes)
+    return set_error(BG_ERR_WORKSPACE, std::string(what) + ": workspace too small");
+  return BG_OK;
+}
+
+Packer::Packer(const BgNamedTensor* weights, int n, void* stream) : st(reinterpret_cast<cudaStream_t>(stream)) {
+  for (int i = 0; i < n; ++i) by_name[weights[i].name] = &weights[i];
+}
+
+const float* Packer::find(const std::string& name, int64_t numel) {
+  auto it = by_name.find(name);
+  if (it == by_name.end()) {
+    if (!err) err = set_error(BG_ERR_MISSING_WEIGHT, "missing weight: " + name);
+    return nullptr;
+  }
+  if (it->second->numel != numel) {
+    if (!err) err = set_error(BG_ERR_BAD_ARG, "weight " + name + " has " + std::to_string(it->second->numel) +
+                                                  " elements, expected " + std::to_string(numel));
+    return nullptr;
+  }
+  return it->second->data;
+}
+
+float* Packer::copy_f32(const std::string& name, int64_t numel) {
+  const float* src = find(name, numel);
+  float* dst = take<float>(numel);
+  if (!dry && src && !err)
+    err = check_cuda(cudaMemcpyAsync(dst, src, numel * sizeof(float), cudaMemcpyDeviceToDevice, st), "copy weight");
+  return dst;
+}
+
+float* Packer::zeros(int64_t numel) {
+  float* dst = take<float>(numel);
+  if (!dry && !err) err = check_cuda(cudaMemsetAsync(dst, 0, numel * sizeof(float), st), "memset");
+  return dst;
+}
+
+int pack_arena(Packer& pk, const std::function<int()>& pack, char** arena, size_t* arena_bytes) {
+  pk.dry = true;
+  pk.off = 0;
+  int s = pack();
+  if (s == 0) {
+    *arena_bytes = pk.off;
+    s = check_cuda(cudaMalloc(reinterpret_cast<void**>(arena), *arena_bytes), "cudaMalloc(weights)");
+  }
+  if (s == 0) {
+    pk.dry = false;
+    pk.base = *arena;
+    pk.off = 0;
+    s = pack();
+  }
+  if (s != 0 && *arena) {
+    cudaFree(*arena);
+    *arena = nullptr;
+  }
+  return s;
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);

@@ -8,9 +8,7 @@
 // Work the reference recomputes every step and we do not: the time-embedding MLP depends only on t -> a 1000 x 768
 // table built at create(); the several per-token embed MLPs of one net are fused into ONE GEMM by concatenating their
 // hidden activations along K (sum of products == product of concatenation).
-#include <map>
 #include <string>
-#include <vector>
 
 #include "../../include/brepgen_b200.h"
 #include "bg_internal.h"
@@ -130,8 +128,6 @@ __global__ void __launch_bounds__(256) mlp_table_kernel(const float* __restrict_
   }
 }
 
-inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
-
 }  // namespace
 
 }  // namespace bg
@@ -160,40 +156,8 @@ struct BgDenoiser {
 
 namespace {
 
-struct Packer {
-  std::map<std::string, const BgNamedTensor*> by_name;
-  char* base = nullptr;
-  size_t off = 0;
-  bool dry = true;
-  cudaStream_t st = nullptr;
-  int err = 0;
-
-  const float* find(const std::string& name, int64_t numel) {
-    auto it = by_name.find(name);
-    if (it == by_name.end()) {
-      if (!err) err = set_error(BG_ERR_MISSING_WEIGHT, "missing weight: " + name);
-      return nullptr;
-    }
-    if (it->second->numel != numel) {
-      if (!err) err = set_error(BG_ERR_BAD_ARG, "weight " + name + " has " + std::to_string(it->second->numel) +
-                                                    " elements, expected " + std::to_string(numel));
-      return nullptr;
-    }
-    return it->second->data;
-  }
-  template <class T>
-  T* take(size_t n) {
-    T* p = dry ? nullptr : reinterpret_cast<T*>(base + off);
-    off += align_up(n * sizeof(T));
-    return p;
-  }
-  float* copy_f32(const std::string& name, int64_t numel) {
-    const float* src = find(name, numel);
-    float* dst = take<float>(numel);
-    if (!dry && src && !err)
-      err = check_cuda(cudaMemcpyAsync(dst, src, numel * sizeof(float), cudaMemcpyDeviceToDevice, st), "copy weight");
-    return dst;
-  }
+struct DPacker : Packer {
+  using Packer::Packer;
   __half* cast_f16(const std::string& name, int64_t numel) {
     const float* src = find(name, numel);
     __half* dst = take<__half>(numel);
@@ -201,9 +165,8 @@ struct Packer {
     return dst;
   }
   // [N][K] fp32 -> fp16 [N][K] (split == 0) or [N][2K] = [W_hi | W_lo]; returns the packed K through *k_out
-  __half* pack_weight(const std::string& name, int N, int K, bool split, int* k_out, int row0 = 0, int rows_total = 0) {
-    const float* src = find(name, (int64_t)(rows_total ? rows_total : N) * K);
-    if (src) src += (size_t)row0 * K;
+  __half* pack_weight(const std::string& name, int N, int K, bool split, int* k_out) {
+    const float* src = find(name, (int64_t)N * K);
     const int kp = split ? 2 * K : K;
     *k_out = kp;
     __half* dst = take<__half>((size_t)N * kp);
@@ -217,7 +180,7 @@ struct Packer {
   }
 };
 
-int pack(BgDenoiser* m, Packer& pk, const float* sincos) {
+int pack(BgDenoiser* m, DPacker& pk, const float* sincos) {
   const KindDef& kd = KINDS[m->kind];
   for (int i = 0; i < NLAYER; ++i) {
     const std::string p = "net.layers." + std::to_string(i) + ".";
@@ -388,21 +351,8 @@ int bg_denoiser_create(int kind, int use_cf, int precision, const BgNamedTensor*
   m->kind = kind;
   m->use_cf = use_cf ? 1 : 0;
   m->precision = precision;
-  Packer pk;
-  for (int i = 0; i < n_weights; ++i) pk.by_name[weights[i].name] = &weights[i];
-  pk.st = reinterpret_cast<cudaStream_t>(stream);
-  pk.dry = true;
-  int s = pack(m, pk, sincos);
-  if (s == 0) {
-    m->arena_bytes = pk.off;
-    s = check_cuda(cudaMalloc(reinterpret_cast<void**>(&m->arena), m->arena_bytes), "cudaMalloc(weights)");
-  }
-  if (s == 0) {
-    pk.dry = false;
-    pk.base = m->arena;
-    pk.off = 0;
-    s = pack(m, pk, sincos);
-  }
+  DPacker pk(weights, n_weights, stream);
+  const int s = pack_arena(pk, [&] { return pack(m, pk, sincos); }, &m->arena, &m->arena_bytes);
   if (s != 0) {
     bg_denoiser_destroy(m);
     return s;
@@ -437,10 +387,9 @@ int bg_denoiser_forward(BgDenoiser* m, const BgDenoiserArgs* a, void* workspace,
   const int B = a->B, S = a->S, E = edge ? a->E : 1;
   const int L = S * E, M = B * L, BS = B * S;
 
-  char* base = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023));
-  Workspace w = carve(base, kind, B, S, edge ? a->E : 0);
-  if (w.bytes + (size_t)(base - reinterpret_cast<char*>(workspace)) > workspace_bytes)
-    return set_error(BG_ERR_WORKSPACE, "denoiser_forward: workspace too small");
+  char* base;
+  BG_TRY(align_workspace(workspace, workspace_bytes, carve(nullptr, kind, B, S, E).bytes, "denoiser_forward", &base));
+  const Workspace w = carve(base, kind, B, S, E);
 
   // 1. conditioning vector per sample: time table row (+ class embedding)
   BG_TRY(launch_cond(st, m->time_table, a->timesteps, a->n_timesteps, m->use_cf ? m->class_table : nullptr,

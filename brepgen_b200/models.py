@@ -36,14 +36,17 @@ def reference_sincos_table(n: int = 1000, dim: int = D) -> torch.Tensor:
     return torch.cat([torch.cos(args), torch.sin(args)], dim=-1)
 
 
-def _register_tree(root: nn.Module, key: str, tensor: torch.Tensor) -> None:
+def _register_tree(root: nn.Module, key: str, tensor: torch.Tensor, buffer: bool = False) -> None:
     parts = key.split(".")
     mod = root
     for p in parts[:-1]:
         if not hasattr(mod, p):
             mod.add_module(p, nn.Module())
         mod = getattr(mod, p)
-    mod.register_parameter(parts[-1], nn.Parameter(tensor, requires_grad=False))
+    if buffer:
+        mod.register_buffer(parts[-1], tensor)
+    else:
+        mod.register_parameter(parts[-1], nn.Parameter(tensor, requires_grad=False))
 
 
 def _default_init(key: str, shape) -> torch.Tensor:
@@ -126,18 +129,11 @@ class _Denoiser(nn.Module):
             self._dirty = False
             return
         self._release()
-        sd = {k: v.detach() for k, v in self.state_dict().items()}
-        for k, v in sd.items():
-            if v.device != device or v.dtype != torch.float32 or not v.is_contiguous():
-                raise RuntimeError(f"parameter {k} must be contiguous fp32 on {device} (call .to(device) first)")
-        names = [k.encode() for k in sd]
-        arr = (_ffi.BgNamedTensor * len(sd))()
-        for i, (k, v) in enumerate(sd.items()):
-            arr[i].name, arr[i].data, arr[i].numel = names[i], v.data_ptr(), v.numel()
+        arr = _ffi.named_tensors(self.state_dict(), device)
         sincos = reference_sincos_table().to(device)
         out = C.c_void_p()
         st = _ffi.current_stream()
-        _ffi.check(_ffi.lib().bg_denoiser_create(_KIND_ID[self.kind], int(self.use_cf), int(self.precision), arr, len(sd),
+        _ffi.check(_ffi.lib().bg_denoiser_create(_KIND_ID[self.kind], int(self.use_cf), int(self.precision), arr, len(arr),
                                                 sincos.data_ptr(), st, C.byref(out)), "bg_denoiser_create")
         torch.cuda.current_stream().synchronize()   # weights / sincos may now be released or modified
         self._handle, self._packed_sig, self._dirty = out, sig, False

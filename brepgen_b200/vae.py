@@ -35,14 +35,8 @@ class _VaeModule(nn.Module):
                 raise NotImplementedError(f"{type(self).__name__}: only {k}={v} (the reference's sample.py config) is built")
         for key, shape in spec:
             if key.endswith(".kernel"):       # fixed resampling taps: a registered buffer, like diffusers' Up/Downsample1d
-                parts = key.split(".")
-                mod = self
-                for p in parts[:-1]:
-                    if not hasattr(mod, p):
-                        mod.add_module(p, nn.Module())
-                    mod = getattr(mod, p)
                 taps = CUBIC_UP_KERNEL if key.endswith("up.kernel") else CUBIC_DOWN_KERNEL
-                mod.register_buffer("kernel", torch.tensor(taps, dtype=torch.float32))
+                _register_tree(self, key, torch.tensor(taps, dtype=torch.float32), buffer=True)
             else:
                 _register_tree(self, key, torch.zeros(shape) if len(shape) == 1 else torch.randn(shape) * 0.02)
         self._handle, self._sig, self._ws = None, None, None
@@ -61,20 +55,14 @@ class _VaeModule(nn.Module):
             pass
 
     def _ensure(self, device):
-        sd = {k: v.detach() for k, v in self.state_dict().items()}
+        sd = self.state_dict()
         sig = tuple((v.data_ptr(), v._version) for v in sd.values())
         if self._handle is not None and sig == self._sig:
             return
         self._release()
-        for k, v in sd.items():
-            if v.device != device or v.dtype != torch.float32 or not v.is_contiguous():
-                raise RuntimeError(f"parameter {k} must be contiguous fp32 on {device} (call .to(device) first)")
-        names = [k.encode() for k in sd]
-        arr = (_ffi.BgNamedTensor * len(sd))()
-        for i, (k, v) in enumerate(sd.items()):
-            arr[i].name, arr[i].data, arr[i].numel = names[i], v.data_ptr(), v.numel()
+        arr = _ffi.named_tensors(sd, device)
         out = C.c_void_p()
-        _ffi.check(_ffi.lib().bg_vae_create(self.kind, arr, len(sd), _ffi.current_stream(), C.byref(out)), "bg_vae_create")
+        _ffi.check(_ffi.lib().bg_vae_create(self.kind, arr, len(arr), _ffi.current_stream(), C.byref(out)), "bg_vae_create")
         torch.cuda.current_stream().synchronize()
         self._handle, self._sig = out, sig
         self._graphs = {}

@@ -178,22 +178,33 @@ def test_decoders_graph_replay_equals_eager():
 
 def test_implicit_convolutions_equal_explicit_im2col():
     """the implicit-GEMM convolutions (TMA boxes of the image per tap) and the explicit im2col gather + GEMM run the same
-    k-block order through the same MMA, so the decoders' outputs are bit-identical; the switch is read at handle creation"""
+    k-block order through the same MMA, so the decoders' and the encoders' outputs are bit-identical; the switch is read at
+    handle creation"""
     import os
-    from brepgen_b200.vae import build_synthetic_decoders
+    from brepgen_b200.spec import edge_encoder_spec, surf_encoder_spec
+    from brepgen_b200.vae import AutoencoderKL1DFastEncode, AutoencoderKLFastEncode, build_synthetic_decoders
     dev = torch.device("cuda")
     zs = torch.randn(37, 3, 4, 4, generator=torch.Generator().manual_seed(3)).cuda()      # 37 * 16 rows: a ragged last tile
     ze = torch.randn(203, 3, 4, generator=torch.Generator().manual_seed(4)).cuda()
+    g = torch.Generator().manual_seed(5)
+    xs = (torch.rand(37, 3, 32, 32, generator=g) * 2 - 1).cuda()   # 4 x 4 at the encoder's conv_out: 37 * 16 rows again
+    xe = (torch.rand(203, 3, 32, generator=g) * 2 - 1).cuda()
     outs = []
     for explicit in (0, 1):
         os.environ["BREPGEN_B200_VAE_IM2COL"] = str(explicit)
         try:
             sv, ev = build_synthetic_decoders(dev)
-            sv.use_graph = ev.use_graph = False
+            es, ee = AutoencoderKLFastEncode(), AutoencoderKL1DFastEncode()
+            es.load_state_dict(synth_state_dict(surf_encoder_spec(), seed=7), strict=False)
+            ee.load_state_dict(synth_state_dict(edge_encoder_spec(), seed=8), strict=False)
+            mods = (sv, ev, es.to(dev).eval(), ee.to(dev).eval())
+            for m in mods:
+                m.use_graph = False
             with torch.no_grad():
-                outs.append((sv(zs), ev(ze)))
+                outs.append([m(x) for m, x in zip(mods, (zs, ze, xs, xe))])
             torch.cuda.synchronize()
         finally:
             os.environ.pop("BREPGEN_B200_VAE_IM2COL", None)
-    assert torch.isfinite(outs[0][0]).all() and torch.isfinite(outs[0][1]).all()
-    assert torch.equal(outs[0][0], outs[1][0]) and torch.equal(outs[0][1], outs[1][1])
+    for implicit, explicit in zip(*outs):
+        assert torch.isfinite(implicit).all()
+        assert torch.equal(implicit, explicit)
