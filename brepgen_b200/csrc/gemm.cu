@@ -10,7 +10,8 @@
 //   warpgroups 1-2 : consumers, one 64-row half of the tile each: 4 x wgmma m64nBNk16 per 64-wide k-block with both
 //                    operands read from shared memory, one k-block in flight while the previous stage is released;
 //                    the epilogue works straight from the accumulator registers while the producer already fills the
-//                    ring for the next tile
+//                    ring for the next tile; the producer also prefetches the tile's residual rows into L2 when it
+//                    starts the tile, so the epilogue's residual reads hit L2 rather than HBM
 // Roofline: tensor-bound; 2*M*N*K flop per launch.
 #include <stdlib.h>
 
@@ -79,6 +80,7 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int m_blk = tile / num_n, n_blk = tile % num_n;
         const int nk = (n_blk * BN < p.n_short) ? p.k_short / BK : num_k;
+        gemm_prefetch_resid<BM, BN>(p, m_blk * BM, n_blk * BN);
         for (int kb = 0; kb < nk; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1);
           uint8_t* sA = smem + stage * C::STAGE_BYTES;

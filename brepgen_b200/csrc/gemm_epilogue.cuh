@@ -44,12 +44,35 @@ __device__ __forceinline__ GemmParams gemm_resolve(const GemmParams& p) {
 }
 
 
+// Warms L2 with the residual rows of the tile [row0, row0 + BM) x [col0, col0 + BN): one bulk prefetch per row, issued
+// by the producer thread when it starts the tile, so the bytes arrive while the tile's MMAs run and the epilogue reads
+// them from L2 instead of HBM.  The range is widened to 16-byte boundaries (the bulk-copy granule); the widened ends lie
+// in granules that hold bytes of the row, so no address outside mapped memory is touched.
+template <int BM, int BN>
+__device__ __forceinline__ void gemm_prefetch_resid(const GemmParams& p, int row0, int col0) {
+  if (!p.resid || p.out_f16) return;
+  const int rows = min(BM, p.M - row0);
+  for (int r = 0; r < rows; ++r) {
+    const uintptr_t a = reinterpret_cast<uintptr_t>(p.resid + (size_t)(row0 + r) * p.ldr + col0);
+    const uintptr_t lo = a & ~uintptr_t(15), hi = (a + BN * sizeof(float) + 15) & ~uintptr_t(15);
+    prefetch_l2_bulk(reinterpret_cast<const void*>(lo), (uint32_t)(hi - lo));
+  }
+}
+
 // One consumer warpgroup, one 64 x BN accumulator tile held in registers in the wgmma m64nBN fp32 layout: warp w of
 // the warpgroup owns rows 16w + lane / 4 (acc[4i], acc[4i + 1]) and 16w + 8 + lane / 4 (acc[4i + 2], acc[4i + 3]) at
 // columns 8i + 2 (lane % 4) + {0, 1}.  Each quad of lanes therefore covers 8 contiguous columns (32 B in fp32) of a row,
 // and the epilogue works on column pairs: float2 loads of bias / residual, float2 or half2 stores.
+//
+// Per row and group of EPI_GROUP column pairs, two passes: the first adds bias, row vector and residual into acc, the
+// second applies ReLU, converts and stores.  `out` and `resid` may be the same array (the in-place residual stream), so
+// the compiler cannot hoist a residual load above a store; with a group's loads ahead of its stores they are in flight
+// together instead of one or two at a time.  Each thread reads only the elements it writes, so the order is safe.  The
+// group size bounds the registers the loads in flight take (the accumulators already hold BN / 2 of them).
+constexpr int EPI_GROUP = 8;
+
 template <int BN>
-__device__ __forceinline__ void gemm_epilogue_regs(const GemmParams& p, const float (&acc)[BN / 2], int row0, int col0,
+__device__ __forceinline__ void gemm_epilogue_regs(const GemmParams& p, float (&acc)[BN / 2], int row0, int col0,
                                                    int warp_in_wg, int lane) {
 #pragma unroll
   for (int hr = 0; hr < 2; ++hr) {
@@ -59,31 +82,40 @@ __device__ __forceinline__ void gemm_epilogue_regs(const GemmParams& p, const fl
                           ? p.rowvec + (size_t)((p.row_map ? p.row_map[row] : row) / p.rows_per_vec) * p.ldv : nullptr;
     const float* rs = (p.resid && !p.out_f16) ? p.resid + (size_t)row * p.ldr : nullptr;
 #pragma unroll
-    for (int i = 0; i < BN / 8; ++i) {
-      const int col = col0 + 8 * i + 2 * (lane & 3);
-      float v0 = acc[4 * i + 2 * hr], v1 = acc[4 * i + 2 * hr + 1];
-      if (p.bias) {
-        const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
-        v0 += b.x;
-        v1 += b.y;
+    for (int g = 0; g < BN / 8; g += EPI_GROUP) {
+#pragma unroll
+      for (int i = g; i < g + EPI_GROUP; ++i) {
+        const int col = col0 + 8 * i + 2 * (lane & 3);
+        float& v0 = acc[4 * i + 2 * hr];
+        float& v1 = acc[4 * i + 2 * hr + 1];
+        if (p.bias) {
+          const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+          v0 += b.x;
+          v1 += b.y;
+        }
+        if (rv) {
+          v0 += __ldg(rv + col);
+          v1 += __ldg(rv + col + 1);
+        }
+        if (rs) {
+          const float2 r = *reinterpret_cast<const float2*>(rs + col);
+          v0 += r.x;
+          v1 += r.y;
+        }
       }
-      if (rv) {
-        v0 += __ldg(rv + col);
-        v1 += __ldg(rv + col + 1);
+#pragma unroll
+      for (int i = g; i < g + EPI_GROUP; ++i) {
+        const int col = col0 + 8 * i + 2 * (lane & 3);
+        float v0 = acc[4 * i + 2 * hr], v1 = acc[4 * i + 2 * hr + 1];
+        if (p.relu) {
+          v0 = fmaxf(v0, 0.f);
+          v1 = fmaxf(v1, 0.f);
+        }
+        if (p.out_f16)
+          *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(p.out) + (size_t)row * p.ldo + col) = pack_half2(v0, v1);
+        else
+          *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + (size_t)row * p.ldo + col) = make_float2(v0, v1);
       }
-      if (rs) {
-        const float2 r = *reinterpret_cast<const float2*>(rs + col);
-        v0 += r.x;
-        v1 += r.y;
-      }
-      if (p.relu) {
-        v0 = fmaxf(v0, 0.f);
-        v1 = fmaxf(v1, 0.f);
-      }
-      if (p.out_f16)
-        *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(p.out) + (size_t)row * p.ldo + col) = pack_half2(v0, v1);
-      else
-        *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + (size_t)row * p.ldo + col) = make_float2(v0, v1);
     }
   }
 }

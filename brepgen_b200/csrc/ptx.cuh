@@ -71,6 +71,11 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
+// bulk prefetch of [p, p + bytes) into L2 (no shared memory, no completion); p and bytes multiples of 16
+__device__ __forceinline__ void prefetch_l2_bulk(const void* p, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(reinterpret_cast<uint64_t>(p)), "r"(bytes) : "memory");
+}
+
 // ---------------------------------------------------------------- register budget of a warpgroup
 template <uint32_t N>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
