@@ -57,6 +57,18 @@ int bg_op_attention(const void* qkv, void* out, int B, int L, const uint8_t* key
   return launch_attention(st, a);
 }
 
+int bg_op_attention_varlen(const void* qkv, void* out, int B, int L, const int* seq_row0, const int* seq_len,
+                           void* stream) {
+  BG_TRY(bg_check_device());
+  BG_REQUIRE(seq_row0 && seq_len, "attention: variable-length mode needs seq_row0 and seq_len");
+  AttnArgs a;
+  a.qkv = reinterpret_cast<const __half*>(qkv);
+  a.out = reinterpret_cast<__half*>(out);
+  a.ldo = 768; a.B = B; a.L = L;
+  a.seq_row0 = seq_row0; a.seq_len = seq_len;
+  return launch_attention(reinterpret_cast<cudaStream_t>(stream), a);
+}
+
 int bg_op_layernorm_f16(const float* x, int ldx, const float* gamma, const float* beta, void* y, int ldy, int rows,
                         int act, void* stream) {
   return launch_layernorm_f16(reinterpret_cast<cudaStream_t>(stream), x, ldx, gamma, beta, reinterpret_cast<__half*>(y),

@@ -14,6 +14,12 @@
 //                      O = O a + P V_j      8 x wgmma m64n64k16, A = P as fp16 straight from the S registers,
 //                                           B = V MN-major SW128 from shared memory
 //                    S, P and O never leave the registers; the two consumer warpgroups interleave on the tensor core.
+// The exponentials cost about as many SM clocks as the MMAs at head dim 64, so within a warpgroup the two overlap:
+// S_{j+1} = Q K_{j+1}^T and O += P_j V_j are issued together, and the softmax of block j + 1 runs while P_j V_j is still
+// on the tensor core (registers for S_{j+1} and the fp16 P_j at once).  Handing the tensor core between the two
+// warpgroups in strict turns (named barriers) measured slower than leaving them to interleave, and is not done.
+// The arithmetic (MMA sequence, max / alpha / exp2 / row-sum order, O *= alpha before O += P V) is that of a plain
+// block-by-block loop: the pipelining changes when instructions run, not what they compute.
 // Fully padded key blocks are skipped through a per-sample block list (result-preserving: their p is exactly 0).
 // Roofline: tensor-bound; 4*L*L*64 flop per (sample, head).
 #include <math.h>
@@ -31,7 +37,7 @@ constexpr int NHEAD = 12;
 constexpr int DMODEL = 768;
 constexpr int BQ = 128;                    // query rows per CTA (two consumer warpgroups of 64)
 constexpr int TILE_BYTES = 128 * DH * 2;   // 16 KB: Q / K / V tile, 128 rows x 128 B
-constexpr int ST = 2;                      // K / V ring depth
+constexpr int ST = 2;                      // K / V ring depth (4 measured no faster)
 constexpr int OFF_Q = 0;
 constexpr int OFF_K = TILE_BYTES;
 constexpr int OFF_V = OFF_K + ST * TILE_BYTES;
@@ -62,6 +68,95 @@ __device__ __forceinline__ float quad_max(float v) {
 __device__ __forceinline__ float quad_sum(float v) {
   v += __shfl_xor_sync(0xffffffffu, v, 1);
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+// stage / phase of one mbarrier ring, advanced in step by its producer and its consumers
+struct Ring {
+  int stage = 0;
+  uint32_t phase = 0;
+  __device__ __forceinline__ void advance() {
+    if (++stage == ST) {
+      stage = 0;
+      phase ^= 1u;
+    }
+  }
+};
+
+__device__ __forceinline__ void issue_qk(float (&sc)[64], uint32_t q_addr, uint32_t k_addr) {
+#pragma unroll
+  for (int k = 0; k < DH / 16; ++k)
+    wgmma_m64n128k16_ss(sc, make_sw128_desc(q_addr + k * 32), make_sw128_desc(k_addr + k * 32), k > 0 ? 1u : 0u);
+  wgmma_commit();
+}
+
+__device__ __forceinline__ void issue_pv(float (&o)[DH / 2], const uint32_t (&pa)[8][4], uint32_t v_addr) {
+#pragma unroll
+  for (int kk = 0; kk < 8; ++kk) wgmma_m64n64k16_rs_bt(o, pa[kk], make_sw128_desc(v_addr + kk * 2048), 1u);
+  wgmma_commit();
+}
+
+// Online softmax of one key block, in place: masks the invalid keys (bit words iw4), updates the running row max and
+// sum, returns the factor alpha that rescales the output rows, and leaves p = exp2(c s - c m) (fp32) in sc.
+__device__ __forceinline__ void softmax_block(float (&sc)[64], const uint32_t* iw4, float (&m_run)[2], float (&l_run)[2],
+                                              float (&alpha)[2], float c, int lane) {
+  const uint4 iw = *reinterpret_cast<const uint4*>(iw4);
+  if ((iw.x | iw.y | iw.z | iw.w) != 0) {
+    const uint32_t inval[4] = {iw.x, iw.y, iw.z, iw.w};
+#pragma unroll
+    for (int i = 0; i < 16; ++i)
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int key = 8 * i + 2 * (lane & 3) + j;
+        if ((inval[key >> 5] >> (key & 31)) & 1u) {
+          sc[4 * i + j] = -INFINITY;
+          sc[4 * i + 2 + j] = -INFINITY;
+        }
+      }
+  }
+  float ref[2];
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    float mx = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) mx = fmaxf(mx, fmaxf(sc[4 * i + 2 * hr], sc[4 * i + 2 * hr + 1]));
+    const float m_new = fmaxf(m_run[hr], quad_max(mx));
+    ref[hr] = m_new == -INFINITY ? 0.f : m_new;        // a row without any valid key so far keeps p = 0
+    alpha[hr] = ex2((m_run[hr] - ref[hr]) * c);         // 0 while the row had no valid key (m_run = -inf)
+    m_run[hr] = m_new;
+    l_run[hr] *= alpha[hr];
+  }
+  const float nm0 = -ref[0] * c, nm1 = -ref[1] * c;
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    const float p0 = ex2(fmaf(sc[4 * i], c, nm0)), p1 = ex2(fmaf(sc[4 * i + 1], c, nm0));
+    const float p2 = ex2(fmaf(sc[4 * i + 2], c, nm1)), p3 = ex2(fmaf(sc[4 * i + 3], c, nm1));
+    l_run[0] += p0 + p1;
+    l_run[1] += p2 + p3;
+    sc[4 * i] = p0;
+    sc[4 * i + 1] = p1;
+    sc[4 * i + 2] = p2;
+    sc[4 * i + 3] = p3;
+  }
+}
+
+__device__ __forceinline__ void scale_o(float (&o)[DH / 2], const float (&alpha)[2]) {
+#pragma unroll
+  for (int i = 0; i < DH / 8; ++i) {
+    o[4 * i] *= alpha[0];
+    o[4 * i + 1] *= alpha[0];
+    o[4 * i + 2] *= alpha[1];
+    o[4 * i + 3] *= alpha[1];
+  }
+}
+
+// the fp16 A fragments of P V: the A fragment of key slice kk (16 keys) is {rows r, r + 8} x {keys 16kk + 2 (lane % 4)
+// + {0, 1}, + 8}, i.e. exactly accumulator columns 2kk and 2kk + 1
+__device__ __forceinline__ void pack_p(uint32_t (&pa)[8][4], const float (&sc)[64]) {
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    pa[i >> 1][(i & 1) * 2] = pack_half2(sc[4 * i], sc[4 * i + 1]);
+    pa[i >> 1][(i & 1) * 2 + 1] = pack_half2(sc[4 * i + 2], sc[4 * i + 3]);
+  }
 }
 
 __global__ void __launch_bounds__(THREADS, 1)
@@ -133,14 +228,14 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParams p) {
     if (warp == 0 && elect_one()) {
       mbar_arrive_expect_tx(q_full, TILE_BYTES);
       tma_load_2d(smem + OFF_Q, &tmQKV, q_full, h * DH, row0 + qgrp * BQ);
-      for (int it = 0; it < nblk; ++it) {
+      Ring r;
+      for (int it = 0; it < nblk; ++it, r.advance()) {
         const int kb = blist ? blist[it] : it;
-        const int s = it % ST;
-        const uint32_t par = ((it / ST) & 1) ^ 1;
-        mbar_wait(&k_empty[s], par);
+        const int s = r.stage;
+        mbar_wait(&k_empty[s], r.phase ^ 1u);
         mbar_arrive_expect_tx(&k_full[s], TILE_BYTES);
         tma_load_2d(smem + OFF_K + s * TILE_BYTES, &tmQKV, &k_full[s], DMODEL + h * DH, row0 + kb * 128);
-        mbar_wait(&v_empty[s], par);
+        mbar_wait(&v_empty[s], r.phase ^ 1u);
         mbar_arrive_expect_tx(&v_full[s], TILE_BYTES);
         tma_load_2d(smem + OFF_V + s * TILE_BYTES, &tmQKV, &v_full[s], 2 * DMODEL + h * DH, row0 + kb * 128);
       }
@@ -163,78 +258,64 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParams p) {
   for (int i = 0; i < DH / 2; ++i) o[i] = 0.f;
 
   mbar_wait(q_full, 0);
-  for (int it = 0; it < nblk; ++it) {
-    const int s = it % ST;
-    const uint32_t par = (it / ST) & 1;
-    float sc[64];
-    mbar_wait(&k_full[s], par);
-    const uint32_t k_addr = smem_u32(smem + OFF_K + s * TILE_BYTES);
+  if (nblk > 0) {
+    const uint32_t k_base = smem_u32(smem + OFF_K), v_base = smem_u32(smem + OFF_V);
+    Ring kr, vr;                 // K_j is consumed in step j, V_j one step later
+    float sc[64], alpha[2];
+    uint32_t pa[8][4];
+
+    // step 0: S_0 alone
+    mbar_wait(&k_full[kr.stage], kr.phase);
     wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < DH / 16; ++k)
-      wgmma_m64n128k16_ss(sc, make_sw128_desc(q_addr + k * 32), make_sw128_desc(k_addr + k * 32), k > 0 ? 1u : 0u);
-    wgmma_commit();
+    issue_qk(sc, q_addr, k_base + kr.stage * TILE_BYTES);
     wgmma_wait<0>();
     wgmma_fence_operand(sc);
-    mbar_arrive(&k_empty[s]);
+    mbar_arrive(&k_empty[kr.stage]);
+    kr.advance();
+    softmax_block(sc, maskw, m_run, l_run, alpha, c, lane);
 
-    const uint4 iw = *reinterpret_cast<const uint4*>(maskw + it * 4);
-    if ((iw.x | iw.y | iw.z | iw.w) != 0) {
-      const uint32_t inval[4] = {iw.x, iw.y, iw.z, iw.w};
-#pragma unroll
-      for (int i = 0; i < 16; ++i)
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          const int key = 8 * i + 2 * (lane & 3) + j;
-          if ((inval[key >> 5] >> (key & 31)) & 1u) {
-            sc[4 * i + j] = -INFINITY;
-            sc[4 * i + 2 + j] = -INFINITY;
-          }
-        }
-    }
-    float ref[2], alpha[2];
-#pragma unroll
-    for (int hr = 0; hr < 2; ++hr) {
-      float mx = -INFINITY;
-#pragma unroll
-      for (int i = 0; i < 16; ++i) mx = fmaxf(mx, fmaxf(sc[4 * i + 2 * hr], sc[4 * i + 2 * hr + 1]));
-      const float m_new = fmaxf(m_run[hr], quad_max(mx));
-      ref[hr] = m_new == -INFINITY ? 0.f : m_new;        // a row without any valid key so far keeps p = 0
-      alpha[hr] = ex2((m_run[hr] - ref[hr]) * c);         // 0 while the row had no valid key (m_run = -inf)
-      m_run[hr] = m_new;
-      l_run[hr] *= alpha[hr];
-    }
-#pragma unroll
-    for (int i = 0; i < DH / 8; ++i) {
-      o[4 * i] *= alpha[0];
-      o[4 * i + 1] *= alpha[0];
-      o[4 * i + 2] *= alpha[1];
-      o[4 * i + 3] *= alpha[1];
-    }
-    // p = exp2(c s - c m), row sums in fp32, and the fp16 A fragments of P V: the A fragment of key slice kk (16 keys)
-    // is {rows r, r + 8} x {keys 16kk + 2 (lane % 4) + {0, 1}, + 8}, i.e. exactly accumulator columns 2kk and 2kk + 1
-    uint32_t pa[8][4];
-    const float nm0 = -ref[0] * c, nm1 = -ref[1] * c;
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const float p0 = ex2(fmaf(sc[4 * i], c, nm0)), p1 = ex2(fmaf(sc[4 * i + 1], c, nm0));
-      const float p2 = ex2(fmaf(sc[4 * i + 2], c, nm1)), p3 = ex2(fmaf(sc[4 * i + 3], c, nm1));
-      l_run[0] += p0 + p1;
-      l_run[1] += p2 + p3;
-      pa[i >> 1][(i & 1) * 2] = pack_half2(p0, p1);
-      pa[i >> 1][(i & 1) * 2 + 1] = pack_half2(p2, p3);
+    // step j: S_j and O += P_{j-1} V_{j-1} on the tensor core; the softmax of S_j runs while P_{j-1} V_{j-1} finishes.
+    // The wait for P_{j-1} V_{j-1} sits at the top of the next step: within one step the compiler would schedule the
+    // exponentials below it, and nothing would overlap.
+#pragma unroll 1
+    for (int it = 1; it < nblk; ++it) {
+      wgmma_wait<0>();
+      wgmma_fence_operand(o);
+      if (it >= 2) {             // P_{it-2} V_{it-2} has finished with its V stage
+        mbar_arrive(&v_empty[vr.stage]);
+        vr.advance();
+      }
+      scale_o(o, alpha);
+      pack_p(pa, sc);
+      mbar_wait(&k_full[kr.stage], kr.phase);
+      mbar_wait(&v_full[vr.stage], vr.phase);
+      wgmma_fence_operand(o);
+      wgmma_fence();
+      issue_qk(sc, q_addr, k_base + kr.stage * TILE_BYTES);
+      issue_pv(o, pa, v_base + vr.stage * TILE_BYTES);
+      wgmma_wait<1>();
+      wgmma_fence_operand(sc);
+      mbar_arrive(&k_empty[kr.stage]);
+      kr.advance();
+      softmax_block(sc, maskw + it * 4, m_run, l_run, alpha, c, lane);
     }
 
-    mbar_wait(&v_full[s], par);
-    const uint32_t v_addr = smem_u32(smem + OFF_V + s * TILE_BYTES);
-    wgmma_fence_operand(o);
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < 8; ++kk) wgmma_m64n64k16_rs_bt(o, pa[kk], make_sw128_desc(v_addr + kk * 2048), 1u);
-    wgmma_commit();
+    // step nblk: O += P_{nblk-1} V_{nblk-1}
     wgmma_wait<0>();
     wgmma_fence_operand(o);
-    mbar_arrive(&v_empty[s]);
+    if (nblk >= 2) {
+      mbar_arrive(&v_empty[vr.stage]);
+      vr.advance();
+    }
+    scale_o(o, alpha);
+    pack_p(pa, sc);
+    mbar_wait(&v_full[vr.stage], vr.phase);
+    wgmma_fence_operand(o);
+    wgmma_fence();
+    issue_pv(o, pa, v_base + vr.stage * TILE_BYTES);
+    wgmma_wait<0>();
+    wgmma_fence_operand(o);
+    mbar_arrive(&v_empty[vr.stage]);
   }
 
 #pragma unroll

@@ -157,6 +157,11 @@ int bg_op_gemm_f16(const void* A, int lda, const void* W, int ldw, int M, int N,
  * (needs scratch_int of B*(5*ceil(L/128)+1) ints: block list, counts and the invalid-key bit words) */
 int bg_op_attention(const void* qkv, void* out, int B, int L, const uint8_t* key_mask, int use_block_list,
                     int* scratch_int, void* stream);
+/* variable-length mode, as the token-compacted denoiser forwards call it: qkv [B*L][2304] and out [B*L][768] as above,
+ * sample b owns rows [seq_row0[b], seq_row0[b] + seq_len[b]) of both, all of them valid (device int32 [B]);
+ * L >= every seq_len[b]; rows outside every sample are not written */
+int bg_op_attention_varlen(const void* qkv, void* out, int B, int L, const int* seq_row0, const int* seq_len,
+                           void* stream);
 int bg_op_layernorm_f16(const float* x, int ldx, const float* gamma, const float* beta, void* y, int ldy, int rows,
                         int act, void* stream);
 int bg_op_cast_f16(const float* x, void* y, int64_t n, void* stream);
