@@ -54,9 +54,13 @@ SIGNATURES = {
     "bg_surf_init": (i32, [vp, vp, vp, vp, vp, i32, vp, vp]),
     "bg_surf_offset_opt": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, f32, f32, f32, f32, f32, vp, vp, vp]),
     "bg_op_gemm_f16": (i32, [vp, i32, vp, i32, i32, i32, i32, vp, i32, i32, i32, vp, vp, i32, vp, i32, i32, vp]),
+    "bg_op_gemm_f16_ex": (i32, [vp, i32, vp, i32, i32, i32, i32, vp, i32, i32, i32, vp, vp, i32, vp, i32, i32,
+                                i32, i32, i32, vp, vp, vp]),
+    "bg_op_conv_f16": (i32, [vp, i32, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp, i32, vp, vp, i32, vp]),
     "bg_op_attention": (i32, [vp, vp, i32, i32, vp, i32, vp, vp]),
     "bg_op_attention_varlen": (i32, [vp, vp, i32, i32, vp, vp, vp]),
     "bg_op_layernorm_f16": (i32, [vp, i32, vp, vp, vp, i32, i32, i32, vp]),
+    "bg_op_layernorm_f16_ex": (i32, [vp, i32, vp, vp, vp, i32, i32, i32, i32, vp, vp]),
     "bg_op_cast_f16": (i32, [vp, vp, i64, vp]),
 }
 

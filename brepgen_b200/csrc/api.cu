@@ -37,6 +37,33 @@ int bg_op_gemm_f16(const void* A, int lda, const void* W, int ldw, int M, int N,
                          reinterpret_cast<const __half*>(W), ldw, M, N, K, ep);
 }
 
+int bg_op_gemm_f16_ex(const void* A, int lda, const void* W, int ldw, int M, int N, int K, void* out, int ldo, int out_f16,
+                      int relu, const float* bias, const float* resid, int ldr, const float* rowvec, int rows_per_vec,
+                      int ldv, int a_kwrap, int n_short, int k_short, const int* m_dev, const int* row_map, void* stream) {
+  BG_TRY(bg_check_device());
+  GemmEpilogue ep;
+  ep.out = out; ep.ldo = ldo; ep.out_f16 = out_f16; ep.relu = relu; ep.bias = bias;
+  ep.resid = resid; ep.ldr = ldr; ep.rowvec = rowvec; ep.rows_per_vec = rows_per_vec; ep.ldv = ldv;
+  ep.a_kwrap = a_kwrap; ep.n_short = n_short; ep.k_short = k_short; ep.m_dev = m_dev; ep.row_map = row_map;
+  return launch_gemm_f16(reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<const __half*>(A), lda,
+                         reinterpret_cast<const __half*>(W), ldw, M, N, K, ep);
+}
+
+int bg_op_conv_f16(const void* x, int ldc, const void* w, int Cout, int N, int H, int W, int C, int taps, int kw,
+                   int lo_plane, int terms, float* out, int ldo, const float* bias, const float* resid, int ldr,
+                   void* stream) {
+  BG_TRY(bg_check_device());
+  BG_REQUIRE(terms >= 1 && terms <= 3, "conv: terms must be 1, 2 or 3");
+  ConvGeom g;
+  g.taps = taps; g.kw = kw; g.C = C; g.W = W; g.H = H; g.N = N; g.lo_plane = lo_plane; g.terms = terms;
+  GemmEpilogue ep;
+  ep.out = out; ep.ldo = ldo; ep.out_f16 = 0; ep.bias = bias; ep.resid = resid; ep.ldr = ldr;
+  ep.conv = g;
+  const int K = terms * taps * C;
+  return launch_gemm_f16(reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<const __half*>(x), ldc,
+                         reinterpret_cast<const __half*>(w), K, N * H * W, Cout, K, ep);
+}
+
 int bg_op_attention(const void* qkv, void* out, int B, int L, const uint8_t* key_mask, int use_block_list,
                     int* scratch_int, void* stream) {
   BG_TRY(bg_check_device());
@@ -73,6 +100,12 @@ int bg_op_layernorm_f16(const float* x, int ldx, const float* gamma, const float
                         int act, void* stream) {
   return launch_layernorm_f16(reinterpret_cast<cudaStream_t>(stream), x, ldx, gamma, beta, reinterpret_cast<__half*>(y),
                               ldy, rows, act);
+}
+
+int bg_op_layernorm_f16_ex(const float* x, int ldx, const float* gamma, const float* beta, void* y, int ldy, int rows,
+                           int act, int lo_offset, const int* rows_dev, void* stream) {
+  return launch_layernorm_f16(reinterpret_cast<cudaStream_t>(stream), x, ldx, gamma, beta, reinterpret_cast<__half*>(y),
+                              ldy, rows, act, lo_offset, rows_dev);
 }
 
 int bg_op_cast_f16(const float* x, void* y, int64_t n, void* stream) {

@@ -153,6 +153,24 @@ int bg_dedup_edges(const float* edgePos, const uint8_t* surf_mask, int B, int S,
 int bg_op_gemm_f16(const void* A, int lda, const void* W, int ldw, int M, int N, int K, void* out, int ldo, int out_f16,
                    int relu, const float* bias, const float* resid, int ldr, const float* rowvec, int rows_per_vec,
                    int ldv, void* stream);
+/* bg_op_gemm_f16 with the modes the denoisers use (test entry point; every extra argument may be 0 / NULL):
+ *   a_kwrap > 0: A has a_kwrap columns and is re-read cyclically along K (column k of the product reads A column
+ *                k % a_kwrap): split-weight GEMMs [W_hi | W_lo] and the compensated [x_hi | x_lo | x_hi] x [W_hi | W_hi | W_lo]
+ *   n_short, k_short: output column tiles below n_short (a multiple of 256) stop after the first k_short columns of K
+ *   m_dev:   device int; only rows below min(M, *m_dev) are computed and written
+ *   row_map: device int [M]; row r adds rowvec[row_map[r] / rows_per_vec] instead of rowvec[r / rows_per_vec] */
+int bg_op_gemm_f16_ex(const void* A, int lda, const void* W, int ldw, int M, int N, int K, void* out, int ldo, int out_f16,
+                      int relu, const float* bias, const float* resid, int ldr, const float* rowvec, int rows_per_vec,
+                      int ldv, int a_kwrap, int n_short, int k_short, const int* m_dev, const int* row_map, void* stream);
+/* Implicit-GEMM convolution (stride 1, zero "same" padding: kw / 2 columns, (taps / kw) / 2 rows), as the VAEs run it
+ * (test entry point).  x: channels-last fp16 image (N, H, W, planes * C) with a pitch of ldc elements per pixel; planes = 2
+ * ([hi | lo]) with lo_plane, else 1.  w: fp16 [Cout][terms * taps * C], k = (term, tap, channel), tap = ky * kw + kx.
+ * terms 1: x_hi w_0;  2: x_hi (w_0 + w_1);  3 with lo_plane: x_hi w_0 + x_lo w_1 + x_hi w_2.
+ * out (fp32, pitch ldo) [N * H * W][Cout] = conv + bias (+ resid, pitch ldr; may alias out).  1-D: H = 1, kw = taps.
+ * Shapes: C and Cout multiples of 64 / 128, W * H divides 128 or is a multiple of it. */
+int bg_op_conv_f16(const void* x, int ldc, const void* w, int Cout, int N, int H, int W, int C, int taps, int kw,
+                   int lo_plane, int terms, float* out, int ldo, const float* bias, const float* resid, int ldr,
+                   void* stream);
 /* qkv fp16 [B*L][2304] -> out fp16 [B*L][768]; key_mask (B,L) or NULL; use_block_list: skip fully padded key blocks
  * (needs scratch_int of B*(5*ceil(L/128)+1) ints: block list, counts and the invalid-key bit words) */
 int bg_op_attention(const void* qkv, void* out, int B, int L, const uint8_t* key_mask, int use_block_list,
@@ -164,6 +182,10 @@ int bg_op_attention_varlen(const void* qkv, void* out, int B, int L, const int* 
                            void* stream);
 int bg_op_layernorm_f16(const float* x, int ldx, const float* gamma, const float* beta, void* y, int ldy, int rows,
                         int act, void* stream);
+/* bg_op_layernorm_f16 plus the split the compensated fc_out reads (test entry point): lo_offset > 0 also writes
+ * fp16(value - fp16(value)) at y[row][lo_offset + c]; rows_dev (device int, may be NULL): only min(rows, *rows_dev) rows */
+int bg_op_layernorm_f16_ex(const float* x, int ldx, const float* gamma, const float* beta, void* y, int ldy, int rows,
+                           int act, int lo_offset, const int* rows_dev, void* stream);
 int bg_op_cast_f16(const float* x, void* y, int64_t n, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
