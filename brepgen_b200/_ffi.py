@@ -62,6 +62,16 @@ SIGNATURES = {
     "bg_op_layernorm_f16": (i32, [vp, i32, vp, vp, vp, i32, i32, i32, vp]),
     "bg_op_layernorm_f16_ex": (i32, [vp, i32, vp, vp, vp, i32, i32, i32, i32, vp, vp]),
     "bg_op_cast_f16": (i32, [vp, vp, i64, vp]),
+    "bg_op_embed_in": (i32, [vp, i32, i32, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp]),
+    "bg_op_ln_silu_head": (i32, [vp, i32, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp]),
+    "bg_op_compact": (i32, [vp, i32, i32, vp, vp, vp, vp, vp]),
+    "bg_op_groupnorm": (i32, [vp, i32, i32, i32, i32, f32, vp, vp, i32, vp, vp, vp, vp]),
+    "bg_op_vae_attention": (i32, [vp, vp, i32, i32, i32, f32, vp]),
+    "bg_op_cubic1d": (i32, [vp, vp, i32, i32, i32, vp, i32, vp]),
+    "bg_op_cast_split": (i32, [vp, vp, i64, i32, vp]),
+    "bg_op_upsample2x_split": (i32, [vp, vp, i32, i32, i32, i32, vp]),
+    "bg_op_postquant": (i32, [vp, vp, vp, vp, i32, i32, vp]),
+    "bg_op_im2col": (i32, [vp, i32, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp]),
 }
 
 _lib: Optional[C.CDLL] = None

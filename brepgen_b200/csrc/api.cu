@@ -112,4 +112,24 @@ int bg_op_cast_f16(const float* x, void* y, int64_t n, void* stream) {
   return launch_cast_f32_to_f16(reinterpret_cast<cudaStream_t>(stream), x, reinterpret_cast<__half*>(y), (size_t)n);
 }
 
+int bg_op_embed_in(const float* x, int ldx, int d_in, const float* W0t, const float* b0, const float* gamma,
+                   const float* beta, void* y, int ldy, int rows, const int* rows_dev, const int* row_map, void* stream) {
+  BG_TRY(bg_check_device());
+  return launch_embed_in(reinterpret_cast<cudaStream_t>(stream), x, ldx, d_in, W0t, b0, gamma, beta,
+                         reinterpret_cast<__half*>(y), ldy, rows, rows_dev, row_map);
+}
+
+int bg_op_ln_silu_head(const float* x, int ldx, const float* gamma, const float* beta, const float* W, const float* bias,
+                       float* out, int d_out, int rows, const int* rows_dev, const int* row_map, void* stream) {
+  BG_TRY(bg_check_device());
+  return launch_ln_silu_head(reinterpret_cast<cudaStream_t>(stream), x, ldx, gamma, beta, W, bias, out, d_out, rows,
+                             rows_dev, row_map);
+}
+
+int bg_op_compact(const uint8_t* mask, int B, int L, int* seq_len, int* seq_row0, int* m_valid, int* row_map,
+                  void* stream) {
+  BG_TRY(bg_check_device());
+  return launch_compact(reinterpret_cast<cudaStream_t>(stream), mask, B, L, seq_len, seq_row0, m_valid, row_map);
+}
+
 }  // extern "C"

@@ -588,6 +588,16 @@ bool conv_implicit_ok(int H, int W, int C) {
   const int hw = H * W;
   return C % 64 == 0 && W <= 128 && 128 % W == 0 && (hw % 128 == 0 || 128 % hw == 0);
 }
+// explicit gather of one fp16 plane (pitch ldin) of N images into the kh x kw im2col matrix A (pitch ldA, Kpad columns)
+int im2col(const Ctx& c, const __half* in, int ldin, __half* A, int ldA, int H, int W, int C, int kh, int kw, int stride,
+           int Kpad) {
+  const size_t rows = c.N * (size_t)(H / stride) * (W / stride);
+  const bool v8 = C % 8 == 0;
+  const auto kernel = v8 ? im2col_kernel<8> : im2col_kernel<1>;
+  const size_t tot = rows * (Kpad / (v8 ? 8 : 1));
+  kernel<<<grid_for(tot), 256, 0, c.st>>>(in, ldin, A, ldA, H, W, C, kh, kw, stride, stride == 1 ? kw / 2 : 0, Kpad, tot);
+  return check_launch("im2col_kernel launch");
+}
 // kh x kw convolution (kh * kw = cv.taps; 1-D: H = 1, kh = 1) of the [hi | lo] fp16 image `in` (N, H, W, 2 * cv.cin) into
 // fp32 (N, H / stride, W / stride, cv.cout_pad).  stride 1: "same" zero padding, an implicit GEMM where the shape allows;
 // stride 2: diffusers Downsample2D(padding=0).  Otherwise the explicit im2col gather into the workspace, then a GEMM.
@@ -599,14 +609,9 @@ int conv(const Ctx& c, const __half* in, int H, int W, int kw, int stride, const
     g.lo_plane = 1; g.terms = c.terms;
     return gemm(c, in, cv, rows, out32, nullptr, resid, g);
   }
-  const bool v8 = cv.cin % 8 == 0;
-  const auto kernel = v8 ? im2col_kernel<8> : im2col_kernel<1>;
-  const size_t tot = rows * (cv.kpad / (v8 ? 8 : 1));
-  for (int part = 0; part < c.terms - 1; ++part) {   // hi plane, then (3-term mode) lo plane of the [hi | lo] activation
-    kernel<<<grid_for(tot), 256, 0, c.st>>>(in + part * cv.cin, 2 * cv.cin, c.w.A + part * cv.kpad, 2 * cv.kpad, H, W, cv.cin,
-                                             cv.taps / kw, kw, stride, stride == 1 ? kw / 2 : 0, cv.kpad, tot);
-    BG_TRY(check_launch("im2col_kernel launch"));
-  }
+  for (int part = 0; part < c.terms - 1; ++part)     // hi plane, then (3-term mode) lo plane of the [hi | lo] activation
+    BG_TRY(im2col(c, in + part * cv.cin, 2 * cv.cin, c.w.A + part * cv.kpad, 2 * cv.kpad, H, W, cv.cin, cv.taps / kw, kw,
+                  stride, cv.kpad));
   return gemm(c, c.w.A, cv, rows, out32, nullptr, resid);
 }
 int groupnorm(const Ctx& c, const float* x, int P, int C, int G, float eps, const Norm& n, int act, const float* resid,
@@ -628,18 +633,47 @@ int cast_split(const Ctx& c, const float* x, __half* y, int C, size_t rows) {
   cast_split_kernel<<<grid_for(tot), 256, 0, c.st>>>(x, y, C, tot);
   return check_launch("cast_split_kernel launch");
 }
+// softmax(q k^T * scale) v over the T positions of each sample, 512 channels in Hh heads: qkv (N*T, 3C) fp16 ->
+// out (N*T, [C hi | C lo]) fp16
+int small_attention(const Ctx& c, const __half* qkv, __half* out, int T, int Hh, float scale) {
+  const int C = 512, dh = C / Hh;
+  const size_t smem = (size_t)(3 * T * C + Hh * T * T) * 4;
+  BG_TRY(ensure_dynamic_smem(reinterpret_cast<const void*>(&small_attention_kernel), 112 * 1024));
+  small_attention_kernel<<<(unsigned)c.N, 256, smem, c.st>>>(qkv, out, T, Hh, dh, scale);
+  return check_launch("small_attention_kernel launch");
+}
 // attention block with residual over the T positions of each sample, 512 channels in Hh heads:
 // x += proj(attention(qkv(GroupNorm(x))))
 int attention(const Ctx& c, const Attn& a, float* x, int T, int G, float eps, int Hh, float scale) {
-  const int C = 512, dh = C / Hh;
+  const int C = 512;
   BG_TRY(groupnorm(c, x, T, C, G, eps, a.gn, 0, nullptr, nullptr, c.w.T));
   BG_TRY(gemm(c, c.w.T, a.qkv, c.N * T, nullptr, c.w.Q, nullptr));
   __half* o = c.w.Q + c.N * (size_t)T * 3 * C;   // [N*T][2C]
-  const size_t smem = (size_t)(3 * T * C + Hh * T * T) * 4;
-  BG_TRY(ensure_dynamic_smem(reinterpret_cast<const void*>(&small_attention_kernel), 112 * 1024));
-  small_attention_kernel<<<(unsigned)c.N, 256, smem, c.st>>>(c.w.Q, o, T, Hh, dh, scale);
-  BG_TRY(check_launch("small_attention_kernel launch"));
+  BG_TRY(small_attention(c, c.w.Q, o, T, Hh, scale));
   return gemm(c, o, a.proj, c.N * T, x, nullptr, x);
+}
+// nearest-2x upsampling of x (N, H, W, C) fp32 into the [hi | lo] fp16 image y (N, 2H, 2W, 2C)
+int upsample2x_split(const Ctx& c, const float* x, __half* y, int H, int W, int C) {
+  const size_t tot = c.N * (size_t)4 * H * W * C;
+  upsample2x_split_kernel<<<grid_for(tot), 256, 0, c.st>>>(x, y, H, W, C, tot);
+  return check_launch("upsample2x_split_kernel launch");
+}
+// cubic 2x resampling along L of x (N, L, C) fp32: up -> y (N, 2L, C), else -> y (N, L / 2, C)
+int cubic1d(const Ctx& c, const float* x, float* y, int L, int C, const float* kern, bool up) {
+  if (up) {
+    const size_t tot = c.N * (size_t)2 * L * C;
+    cubic_up1d_kernel<<<grid_for(tot), 256, 0, c.st>>>(x, y, L, C, kern, tot);
+    return check_launch("cubic_up1d_kernel launch");
+  }
+  const size_t tot = c.N * (size_t)(L / 2) * C;
+  cubic_down1d_kernel<<<grid_for(tot), 256, 0, c.st>>>(x, y, L, C, kern, tot);
+  return check_launch("cubic_down1d_kernel launch");
+}
+// z (N, 3, P) fp32 -> y (N, P, [3 hi | 3 lo]) fp16, y = W z + b (post_quant_conv; the identity for the encoders)
+int postquant(const Ctx& c, const float* z, const float* w, const float* b, __half* y, int P) {
+  const int N = (int)c.N;
+  postquant_kernel<<<(N * P + 255) / 256, 256, 0, c.st>>>(z, w, b, y, N, P);
+  return check_launch("postquant_kernel launch");
 }
 
 // x (in place, fp32 [N, H*H, Cout] in *px): diffusers ResnetBlock2D without time embedding
@@ -702,9 +736,7 @@ int mid1d(const Ctx& c, const BgVae* m, float** px, float** pfree) {
 
 // in (N, 3, H*W) fp32 -> 1x1 post_quant_conv (the identity for the encoders) into [hi | lo] fp16 -> conv_in -> x
 int stem(const Ctx& c, const BgVae* m, const float* in, int H, int W, float* x) {
-  const int N = (int)c.N;
-  postquant_kernel<<<(N * H * W + 255) / 256, 256, 0, c.st>>>(in, m->pq_w, m->pq_b, c.w.T, N, H * W);
-  BG_TRY(check_launch("postquant_kernel launch"));
+  BG_TRY(postquant(c, in, m->pq_w, m->pq_b, c.w.T, H * W));
   return conv(c, c.w.T, H, W, 3, 1, m->conv_in, x, nullptr);
 }
 // x -> GroupNorm + SiLU -> conv_out -> out (N, 3, H*W) fp32: the first three channels (decoders) or the mode of
@@ -744,9 +776,7 @@ int run_vae(const BgVae* m, const float* in, int N, int hw, float* out, void* wo
         for (int j = 0; j < 3; ++j) BG_TRY(resnet2d(c, m->s_up[i][j], &x, &spare, H));
         if (i < 3) {   // nearest 2x into the [hi | lo] input of the upsampler's convolution
           const Conv& uc = m->s_upconv[i];
-          const size_t tot = c.N * (size_t)4 * H * H * uc.cin;
-          upsample2x_split_kernel<<<grid_for(tot), 256, 0, c.st>>>(x, c.w.T, H, H, uc.cin, tot);
-          BG_TRY(check_launch("upsample2x_split_kernel launch"));
+          BG_TRY(upsample2x_split(c, x, c.w.T, H, H, uc.cin));
           H *= 2;
           BG_TRY(conv(c, c.w.T, H, H, 3, 1, uc, spare, nullptr));
           std::swap(x, spare);
@@ -758,10 +788,7 @@ int run_vae(const BgVae* m, const float* in, int N, int hw, float* out, void* wo
       BG_TRY(mid1d(c, m, &x, &spare));
       for (int i = 0; i < 3; ++i) {
         for (int j = 0; j < 3; ++j) BG_TRY(resconv1d(c, m->e_up[i][j], &x, &spare, L));
-        const int C = m->e_up[i][2].c2.cout;
-        const size_t tot = c.N * (size_t)2 * L * C;
-        cubic_up1d_kernel<<<grid_for(tot), 256, 0, c.st>>>(x, spare, L, C, m->up_kernel, tot);
-        BG_TRY(check_launch("cubic_up1d_kernel launch"));
+        BG_TRY(cubic1d(c, x, spare, L, m->e_up[i][2].c2.cout, m->up_kernel, true));
         std::swap(x, spare);
         L *= 2;
       }
@@ -783,10 +810,7 @@ int run_vae(const BgVae* m, const float* in, int N, int hw, float* out, void* wo
     default:  // edge encoder
       BG_TRY(stem(c, m, in, 1, L, x));
       for (int i = 0; i < 3; ++i) {
-        const int C = m->e_down[i][0].c1.cin;
-        const size_t tot = c.N * (size_t)(L / 2) * C;
-        cubic_down1d_kernel<<<grid_for(tot), 256, 0, c.st>>>(x, spare, L, C, m->down_kernel, tot);
-        BG_TRY(check_launch("cubic_down1d_kernel launch"));
+        BG_TRY(cubic1d(c, x, spare, L, m->e_down[i][0].c1.cin, m->down_kernel, false));
         std::swap(x, spare);
         L /= 2;
         for (int j = 0; j < 3; ++j) BG_TRY(resconv1d(c, m->e_down[i][j], &x, &spare, L));
@@ -794,6 +818,14 @@ int run_vae(const BgVae* m, const float* in, int N, int hw, float* out, void* wo
       BG_TRY(mid1d(c, m, &x, &spare));
       return head(c, m, x, 1, L, out);
   }
+}
+
+// stream and sample count of a unit-level entry point (no workspace)
+Ctx op_ctx(int N, void* stream) {
+  Ctx c{};
+  c.st = reinterpret_cast<cudaStream_t>(stream);
+  c.N = (size_t)N;
+  return c;
 }
 
 }  // namespace
@@ -853,6 +885,62 @@ int bg_vae_encode(BgVae* m, const float* xin, int N, int hw, float* out, void* w
   BG_REQUIRE(m->kind == 2 ? (hw == 8 || hw == 16 || hw == 24 || hw == 32) : hw == 32,
              "vae_encode: input extent must be 8/16/24/32 (surface) or 32 (edge)");
   return run_vae(m, xin, N, hw, out, workspace, workspace_bytes, stream, "vae_encode");
+}
+
+// ---- unit-level entry points: the networks' own launch code on caller-owned buffers
+int bg_op_groupnorm(const float* x, int N, int P, int C, int G, float eps, const float* gamma, const float* beta, int act,
+                    const float* resid, float* out32, void* out16, void* stream) {
+  BG_TRY(bg_check_device());
+  const int cpg = G > 0 ? C / G : 0;
+  BG_REQUIRE(x && gamma && beta && (out32 || out16) && N > 0 && P > 0 && C > 0 && C <= 1024 && C % 32 == 0 && cpg > 0 &&
+                 C % G == 0 && (cpg > 32 ? cpg % 32 == 0 : 32 % cpg == 0) && act >= 0 && act <= 2,
+             "groupnorm: bad arguments");
+  Norm n;
+  n.g = const_cast<float*>(gamma);
+  n.b = const_cast<float*>(beta);
+  return groupnorm(op_ctx(N, stream), x, P, C, G, eps, n, act, resid, out32, reinterpret_cast<__half*>(out16));
+}
+
+int bg_op_vae_attention(const void* qkv, void* out, int N, int T, int Hh, float scale, void* stream) {
+  BG_TRY(bg_check_device());
+  BG_REQUIRE(qkv && out && N > 0 && T > 0 && Hh > 0 && 512 % Hh == 0 && T * T * Hh <= 256, "vae_attention: bad arguments");
+  return small_attention(op_ctx(N, stream), reinterpret_cast<const __half*>(qkv), reinterpret_cast<__half*>(out), T, Hh,
+                         scale);
+}
+
+int bg_op_cubic1d(const float* x, float* y, int N, int L, int C, const float* kernel8, int up, void* stream) {
+  BG_TRY(bg_check_device());
+  BG_REQUIRE(x && y && kernel8 && N > 0 && L >= 4 && C > 0 && (up || L % 2 == 0), "cubic1d: bad arguments");
+  return cubic1d(op_ctx(N, stream), x, y, L, C, kernel8, up != 0);
+}
+
+int bg_op_cast_split(const float* x, void* y, int64_t rows, int C, void* stream) {
+  BG_TRY(bg_check_device());
+  BG_REQUIRE(x && y && rows > 0 && C > 0, "cast_split: bad arguments");
+  return cast_split(op_ctx(1, stream), x, reinterpret_cast<__half*>(y), C, (size_t)rows);
+}
+
+int bg_op_upsample2x_split(const float* x, void* y, int N, int H, int W, int C, void* stream) {
+  BG_TRY(bg_check_device());
+  BG_REQUIRE(x && y && N > 0 && H > 0 && W > 0 && C > 0, "upsample2x_split: bad arguments");
+  return upsample2x_split(op_ctx(N, stream), x, reinterpret_cast<__half*>(y), H, W, C);
+}
+
+int bg_op_postquant(const float* z, const float* w, const float* b, void* y, int N, int P, void* stream) {
+  BG_TRY(bg_check_device());
+  BG_REQUIRE(z && w && b && y && N > 0 && P > 0, "postquant: bad arguments");
+  return postquant(op_ctx(N, stream), z, w, b, reinterpret_cast<__half*>(y), P);
+}
+
+int bg_op_im2col(const void* in, int ldin, void* A, int ldA, int N, int H, int W, int C, int kh, int kw, int stride,
+                 int Kpad, void* stream) {
+  BG_TRY(bg_check_device());
+  BG_REQUIRE(in && A && N > 0 && H > 0 && W > 0 && C > 0 && kh > 0 && kw > 0 && (stride == 1 || stride == 2) &&
+                 H >= stride && W >= stride && Kpad >= kh * kw * C && ldin >= C && ldA >= Kpad &&
+                 (C % 8 != 0 || (ldin % 8 == 0 && ldA % 8 == 0 && Kpad % 8 == 0)),
+             "im2col: bad arguments");
+  return im2col(op_ctx(N, stream), reinterpret_cast<const __half*>(in), ldin, reinterpret_cast<__half*>(A), ldA, H, W, C,
+                kh, kw, stride, Kpad);
 }
 
 }  // extern "C"

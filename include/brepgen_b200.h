@@ -187,6 +187,42 @@ int bg_op_layernorm_f16(const float* x, int ldx, const float* gamma, const float
 int bg_op_layernorm_f16_ex(const float* x, int ldx, const float* gamma, const float* beta, void* y, int ldy, int rows,
                            int act, int lo_offset, const int* rows_dev, void* stream);
 int bg_op_cast_f16(const float* x, void* y, int64_t n, void* stream);
+/* The denoisers' CUDA-core ends (test entry points), with token compaction's rows_dev (device int: only
+ * min(rows, *rows_dev) rows) and row_map (device int [rows]), both may be NULL.
+ * embed_in:     y[r] (fp16, pitch ldy) = SiLU(LayerNorm(x[row_map[r]][0:d_in] W0t + b0)) (eps 1e-5); W0t [d_in][768]
+ * ln_silu_head: out[row_map[r]][0:d_out] = SiLU(LayerNorm(x[r][0:768])) W^T + bias (fp32); W [d_out][768], d_out <= 64
+ * compact:      mask (B, L), nonzero = padded -> seq_len[b] valid tokens, seq_row0[b] = exclusive prefix sum,
+ *               *m_valid = total, row_map[seq_row0[b] + i] = b * L + (token of the i-th valid one of sample b) */
+int bg_op_embed_in(const float* x, int ldx, int d_in, const float* W0t, const float* b0, const float* gamma,
+                   const float* beta, void* y, int ldy, int rows, const int* rows_dev, const int* row_map, void* stream);
+int bg_op_ln_silu_head(const float* x, int ldx, const float* gamma, const float* beta, const float* W, const float* bias,
+                       float* out, int d_out, int rows, const int* rows_dev, const int* row_map, void* stream);
+int bg_op_compact(const uint8_t* mask, int B, int L, int* seq_len, int* seq_row0, int* m_valid, int* row_map,
+                  void* stream);
+/* The VAEs' CUDA-core kernels through the networks' own launch code (test entry points).  Activations are channels-last
+ * fp32; "[hi | lo]" is an fp16 pair per value, hi = fp16(v), lo = fp16(v - hi), stored as the two halves of each row.
+ * groupnorm:        x (N, P, C) -> act(GroupNorm(x) * gamma + beta) (+ resid, which may alias out32) into out32 (N, P, C)
+ *                   and / or out16 (N, P, [C hi | C lo]); act 0 none, 1 SiLU, 2 GELU (erf); C <= 1024, C / G a power of
+ *                   two up to 32 or a multiple of 32
+ * vae_attention:    qkv (N*T, [q | k | v]) fp16, 512 channels in Hh heads -> out (N*T, [512 hi | 512 lo]) =
+ *                   softmax(q k^T * scale) v per head; T * T * Hh <= 256
+ * cubic1d:          diffusers cubic Upsample1d (up: (N, L, C) -> (N, 2L, C)) / Downsample1d ((N, L, C) -> (N, L / 2, C))
+ *                   with the 8-tap kernel8 and reflect padding
+ * cast_split:       x (rows, C) -> (rows, [C hi | C lo])
+ * upsample2x_split: nearest 2x, x (N, H, W, C) -> (N, 2H, 2W, [C hi | C lo])
+ * postquant:        1x1 convolution 3 -> 3, z (N, 3, P) -> (N, P, [3 hi | 3 lo]) = w z + b, w [3][3]
+ * im2col:           in (N, H, W, C) fp16 (pitch ldin per pixel) -> A (N * H/stride * W/stride, Kpad) (pitch ldA) with
+ *                   k = (ky * kw + kx) * C + c, zero for k >= kh * kw * C; stride 1: "same" zero padding, stride 2: zero
+ *                   padding on the right / bottom only (diffusers Downsample2D(padding=0)) */
+int bg_op_groupnorm(const float* x, int N, int P, int C, int G, float eps, const float* gamma, const float* beta, int act,
+                    const float* resid, float* out32, void* out16, void* stream);
+int bg_op_vae_attention(const void* qkv, void* out, int N, int T, int Hh, float scale, void* stream);
+int bg_op_cubic1d(const float* x, float* y, int N, int L, int C, const float* kernel8, int up, void* stream);
+int bg_op_cast_split(const float* x, void* y, int64_t rows, int C, void* stream);
+int bg_op_upsample2x_split(const float* x, void* y, int N, int H, int W, int C, void* stream);
+int bg_op_postquant(const float* z, const float* w, const float* b, void* y, int N, int P, void* stream);
+int bg_op_im2col(const void* in, int ldin, void* A, int ldA, int N, int H, int W, int C, int kh, int kw, int stride,
+                 int Kpad, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Post-decode geometry glue (SURVEY.md 8(f) row 3): the numeric cores of the per-CAD post-processing between the VAE
