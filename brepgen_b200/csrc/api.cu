@@ -72,6 +72,8 @@ int bg_op_attention(const void* qkv, void* out, int B, int L, const uint8_t* key
   a.qkv = reinterpret_cast<const __half*>(qkv);
   a.out = reinterpret_cast<__half*>(out);
   a.ldo = 768; a.B = B; a.L = L; a.key_mask = key_mask;
+  // checked before the block list is built, so that a rejected call launches nothing
+  BG_REQUIRE(L <= ATTN_MAX_L, "attention: sequence longer than 8192 tokens is not supported");
   if (use_block_list && key_mask) {
     BG_REQUIRE(scratch_int != nullptr, "attention: block list needs scratch_int");
     const int nkb = (L + 127) / 128;

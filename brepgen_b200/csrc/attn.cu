@@ -43,7 +43,7 @@ constexpr int OFF_K = TILE_BYTES;
 constexpr int OFF_V = OFF_K + ST * TILE_BYTES;
 constexpr int OFF_BAR = OFF_V + ST * TILE_BYTES;
 constexpr int OFF_MASKW = OFF_BAR + 256;   // invalid-key bit words: 4 per key block, MAX_KB blocks
-constexpr int MAX_KB = 64;                 // L <= 8192
+constexpr int MAX_KB = ATTN_MAX_L / 128;   // 64 key blocks: L <= 8192
 constexpr int SMEM_BYTES = OFF_MASKW + MAX_KB * 16 + 1024;
 constexpr int THREADS = 384;
 constexpr int CONSUMER_THREADS = 256;
@@ -374,7 +374,7 @@ __global__ void block_list_kernel(const uint8_t* __restrict__ key_mask, int L, i
 int launch_attention(cudaStream_t st, const AttnArgs& a) {
   BG_REQUIRE(a.qkv && a.out && a.B > 0 && a.L > 0, "attention: bad arguments");
   BG_REQUIRE(a.ldo % 8 == 0, "attention: output pitch must be a multiple of 8");
-  BG_REQUIRE(a.L <= 128 * MAX_KB, "attention: sequence longer than 8192 tokens is not supported");
+  BG_REQUIRE(a.L <= ATTN_MAX_L, "attention: sequence longer than 8192 tokens is not supported");
   BG_REQUIRE((a.blk_list == nullptr) == (a.blk_count == nullptr), "attention: blk_list and blk_count go together");
   CUtensorMap tm;
   BG_REQUIRE((a.seq_row0 == nullptr) == (a.seq_len == nullptr), "attention: seq_row0 and seq_len go together");

@@ -139,6 +139,7 @@ struct AttnArgs {
   const int* seq_row0 = nullptr;
   const int* seq_len = nullptr;
 };
+constexpr int ATTN_MAX_L = 8192;   // longest sequence launch_attention takes (64 key blocks of mask words in shared memory)
 int launch_attention(cudaStream_t st, const AttnArgs& a);
 // builds blk_list/blk_count from key_mask ([B,L]); nkb = ceil(L/128)
 int launch_build_block_list(cudaStream_t st, const uint8_t* key_mask, int B, int L, int* blk_list, int* blk_count,
