@@ -34,11 +34,16 @@ SIGNATURES = {
     "bg_denoiser_workspace_bytes": (sz, [vp, i32, i32, i32]),
     "bg_denoiser_forward": (i32, [vp, C.POINTER(BgDenoiserArgs), vp, sz, vp]),
     "bg_vae_create": (i32, [i32, C.POINTER(BgNamedTensor), i32, vp, C.POINTER(vp)]),
+    "bg_vae_create_ex": (i32, [i32, i32, C.POINTER(BgNamedTensor), i32, vp, C.POINTER(vp)]),
     "bg_vae_destroy": (None, [vp]),
     "bg_vae_workspace_bytes": (sz, [vp, i32]),
     "bg_vae_decode": (i32, [vp, vp, i32, vp, vp, sz, vp]),
     "bg_vae_decode_hw": (i32, [vp, vp, i32, i32, vp, vp, sz, vp]),
     "bg_vae_encode": (i32, [vp, vp, i32, i32, vp, vp, sz, vp]),
+    "bg_vae_encode_moments": (i32, [vp, vp, i32, i32, vp, vp, sz, vp]),
+    "bg_vae_posterior": (i32, [vp, vp, i32, i32, i32, vp, vp, vp]),
+    "bg_vae_reconstruct_workspace_bytes": (sz, [vp, vp, i32]),
+    "bg_vae_reconstruct": (i32, [vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, sz, vp]),
     "bg_ddpm_step": (i32, [vp, vp, f32, vp, vp, vp, u64, u64, i64, f32, f32, f32, f32, f32, f32, vp]),
     "bg_ddpm_step_tab": (i32, [vp, vp, f32, vp, vp, u64, u64, u64, i64, vp, vp, f32, vp]),
     "bg_step_advance": (i32, [vp, i32, vp, vp, vp]),

@@ -12,6 +12,7 @@
 // express (3 input channels, 3 x 3 / 24 x 24 extents, stride-2 encoder convolutions) keep the explicit gather.  The GEMM
 // epilogue adds bias and the residual; GroupNorm + SiLU/GELU (+ residual) is one CTA-per-sample kernel; nearest-2x
 // upsampling is one gather into the next convolution's input; the tiny attentions run on CUDA cores.
+#include <algorithm>
 #include <string>
 #include <type_traits>
 #include <utility>
@@ -294,6 +295,74 @@ __global__ void quant_mode_kernel(const float* __restrict__ h, int ld, const flo
   out[i] = acc;
 }
 
+// Posterior of the encoders' latent: diffusers DiagonalGaussianDistribution over quant_conv(encoder(x)).  One warp per
+// sample, lane <-> latent position (p = lane, lane + 32, ...).  The six moment channels are computed here from the conv_out
+// rows h (N*P, pitch ld) by quant_conv when wq != null -- the fmaf order of quant_mode_kernel, so the mean half is
+// bit-identical to the mode bg_vae_encode writes -- or read from mom_in (N, 6, P).  Outputs, each optional:
+//   moments (N, 6, P) raw, diffusers' channel order: mean = channels 0-2, logvar = 3-5
+//   z (N, 3, P) = mean + exp(0.5 clamp(logvar, -30, 20)) * noise, noise (N, 3, P); noise == null: z = mean
+//   kl (N) = 0.5 sum_{c,p} (mean^2 + var - 1 - logvar), var = exp(clamped logvar): lane partials, then a fixed xor tree
+// deterministic != 0: std = var = 0, so z = mean and kl = 0 (diffusers' kl() returns 0 for a deterministic posterior).
+__global__ void posterior_kernel(const float* __restrict__ h, int ld, const float* __restrict__ wq, const float* __restrict__ bq,
+                                 const float* __restrict__ mom_in, const float* __restrict__ noise, int N, int P,
+                                 int deterministic, float* __restrict__ moments, float* __restrict__ z, float* __restrict__ kl) {
+  const int n = (int)((blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (n >= N) return;                      // whole warps: blockDim is a multiple of 32
+  float part = 0.f;
+  for (int p = lane; p < P; p += 32) {
+    float m[6];
+    if (wq) {
+      const float* hr = h + ((size_t)n * P + p) * ld;
+#pragma unroll
+      for (int co = 0; co < 6; ++co) {
+        float acc = bq[co];
+#pragma unroll
+        for (int ci = 0; ci < 6; ++ci) acc = fmaf(wq[co * 6 + ci], hr[ci], acc);
+        m[co] = acc;
+      }
+    } else {
+#pragma unroll
+      for (int co = 0; co < 6; ++co) m[co] = mom_in[((size_t)n * 6 + co) * P + p];
+    }
+    if (moments) {
+#pragma unroll
+      for (int co = 0; co < 6; ++co) moments[((size_t)n * 6 + co) * P + p] = m[co];
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const float logvar = fminf(fmaxf(m[3 + c], -30.f), 20.f);
+      const float sd = deterministic ? 0.f : expf(0.5f * logvar), var = deterministic ? 0.f : expf(logvar);
+      const size_t o = ((size_t)n * 3 + c) * P + p;
+      if (z) z[o] = noise ? fmaf(sd, noise[o], m[c]) : m[c];
+      part += m[c] * m[c] + var - 1.f - logvar;
+    }
+  }
+  if (!kl) return;
+  for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+  if (lane == 0) kl[n] = deterministic ? 0.f : 0.5f * part;
+}
+
+// per-sample reconstruction error: mse[n] = mean over the cnt values of sample n of (a - b)^2.  One 256-thread CTA per
+// sample: strided fp32 partial sums, a fixed shuffle tree per warp, then the 8 warp sums in order (no atomics).
+__global__ void __launch_bounds__(256) sample_mse_kernel(const float* __restrict__ a, const float* __restrict__ b, int cnt,
+                                                         float* __restrict__ mse) {
+  __shared__ float s_part[8];
+  const size_t base = (size_t)blockIdx.x * cnt;
+  float s = 0.f;
+  for (int i = threadIdx.x; i < cnt; i += 256) {
+    const float d = a[base + i] - b[base + i];
+    s = fmaf(d, d, s);
+  }
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t = 0.f;
+    for (int w = 0; w < 8; ++w) t += s_part[w];
+    mse[blockIdx.x] = t / (float)cnt;
+  }
+}
+
 // conv_out result (N*P, ld) fp32 -> out (N, 3, P) fp32 (first three channels)
 __global__ void slice_out_kernel(const float* __restrict__ h, int ld, float* __restrict__ out, int N, int P) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -555,12 +624,20 @@ VaeWs carve_vae(char* base, int kind, size_t N) {
   return w;
 }
 
+// the encoders' posterior tail (bg_vae_encode_moments / bg_vae_reconstruct): posterior_kernel's inputs and outputs, written
+// in place of the mode
+struct Tail {
+  const float* noise = nullptr;
+  float *moments = nullptr, *z = nullptr, *kl = nullptr;
+};
+
 struct Ctx {
   cudaStream_t st;
   size_t N;
   VaeWs w;
   int terms = 3;
   int implicit = 1;
+  const Tail* tail = nullptr;   // encoders: the posterior tail instead of the mode
 };
 
 // out = A * cv^T + bias (+ resid).  A is [rows][2 * cv.kpad] fp16 = [A_hi | A_lo] read cyclically along K:
@@ -739,12 +816,25 @@ int stem(const Ctx& c, const BgVae* m, const float* in, int H, int W, float* x) 
   BG_TRY(postquant(c, in, m->pq_w, m->pq_b, c.w.T, H * W));
   return conv(c, c.w.T, H, W, 3, 1, m->conv_in, x, nullptr);
 }
+// posterior_kernel over the N samples of c: moments from quant_conv(h) (wq != null) or from mom_in (N, 6, P)
+int posterior(const Ctx& c, const float* h, int ld, const float* wq, const float* bq, const float* mom_in, const Tail& t,
+              int P, int deterministic) {
+  posterior_kernel<<<(unsigned)((c.N * 32 + 255) / 256), 256, 0, c.st>>>(h, ld, wq, bq, mom_in, t.noise, (int)c.N, P,
+                                                                        deterministic, t.moments, t.z, t.kl);
+  return check_launch("posterior_kernel launch");
+}
+int sample_mse(const Ctx& c, const float* a, const float* b, int cnt, float* mse) {
+  sample_mse_kernel<<<(unsigned)c.N, 256, 0, c.st>>>(a, b, cnt, mse);
+  return check_launch("sample_mse_kernel launch");
+}
+
 // x -> GroupNorm + SiLU -> conv_out -> out (N, 3, H*W) fp32: the first three channels (decoders) or the mode of
-// quant_conv over the six moment channels (encoders)
+// quant_conv over the six moment channels (encoders; with c.tail, the posterior tail instead and `out` is not written)
 int head(const Ctx& c, const BgVae* m, const float* x, int H, int W, float* out) {
   const int N = (int)c.N, P = H * W, ld = m->conv_out.cout_pad;
   BG_TRY(groupnorm(c, x, P, m->conv_out.cin, 32, 1e-6f, m->norm_out, 1, nullptr, nullptr, c.w.T));
   BG_TRY(conv(c, c.w.T, H, W, 3, 1, m->conv_out, c.w.H, nullptr));
+  if (m->kind >= 2 && c.tail) return posterior(c, c.w.H, ld, m->q_w, m->q_b, nullptr, *c.tail, P, 0);
   if (m->kind >= 2) {
     quant_mode_kernel<<<(N * 3 * P + 255) / 256, 256, 0, c.st>>>(c.w.H, ld, m->q_w, m->q_b, out, N, P);
     return check_launch("quant_mode_kernel launch");
@@ -755,12 +845,13 @@ int head(const Ctx& c, const BgVae* m, const float* x, int H, int W, float* out)
 
 // the whole network of handle m on N inputs of extent hw (latent side for the decoders, image side for the encoders)
 int run_vae(const BgVae* m, const float* in, int N, int hw, float* out, void* workspace, size_t workspace_bytes,
-            void* stream, const char* what) {
+            void* stream, const char* what, const Tail* tail = nullptr) {
   Ctx c;
   c.st = reinterpret_cast<cudaStream_t>(stream);
   c.N = (size_t)N;
   c.terms = m->terms;
   c.implicit = m->implicit;
+  c.tail = tail;
   char* base;
   BG_TRY(align_workspace(workspace, workspace_bytes, carve_vae(nullptr, m->kind, c.N).bytes, what, &base));
   c.w = carve_vae(base, m->kind, c.N);
@@ -833,7 +924,12 @@ Ctx op_ctx(int N, void* stream) {
 extern "C" {
 
 int bg_vae_create(int kind, const BgNamedTensor* weights, int n_weights, void* stream, BgVae** out) {
-  BG_REQUIRE(kind >= 0 && kind <= 3 && weights && n_weights > 0 && out, "vae_create: bad arguments");
+  return bg_vae_create_ex(kind, 0, weights, n_weights, stream, out);
+}
+
+int bg_vae_create_ex(int kind, int terms, const BgNamedTensor* weights, int n_weights, void* stream, BgVae** out) {
+  BG_REQUIRE(kind >= 0 && kind <= 3 && (terms == 0 || terms == 2 || terms == 3) && weights && n_weights > 0 && out,
+             "vae_create: bad arguments");
   BG_TRY(bg_check_device());
   BgVae* m = new BgVae();
   m->kind = kind;
@@ -843,8 +939,10 @@ int bg_vae_create(int kind, const BgNamedTensor* weights, int n_weights, void* s
   //                                           and no lo plane in the im2col matrices
   // Relative L2 errors against the fp32 oracle (bar 1e-3), measured on an H100 with 3 / 2 terms: surface decoder 9.4e-5 /
   // 1.3e-3, edge decoder 3.6e-5 / 4.1-4.3e-4, encoders <= 1.1e-4 / 6.4-9.0e-4.  So the edge decoder uses 2 terms (a third
-  // less GEMM work); the surface decoder, over the bar with 2, and the encoders, close to it, keep 3.
-  m->terms = kind == 1 ? 2 : 3;
+  // less GEMM work); the surface decoder, over the bar with 2, and the encoders, close to it, keep 3.  terms != 0 overrides
+  // the default: the full auto-encoders' edge decoder takes 3, since the two-term error depends on the weights and reaches
+  // 1.1e-3 on some draws.
+  m->terms = terms ? terms : (kind == 1 ? 2 : 3);
   if (const char* e = getenv("BREPGEN_B200_VAE_IM2COL")) m->implicit = atoi(e) ? 0 : 1;
   VPacker pk(weights, n_weights, stream, m->terms);
   const int s = pack_arena(pk, [&] { return kind >= 2 ? pack_encoder(m, pk) : pack_decoder(m, pk); }, &m->arena,
@@ -885,6 +983,60 @@ int bg_vae_encode(BgVae* m, const float* xin, int N, int hw, float* out, void* w
   BG_REQUIRE(m->kind == 2 ? (hw == 8 || hw == 16 || hw == 24 || hw == 32) : hw == 32,
              "vae_encode: input extent must be 8/16/24/32 (surface) or 32 (edge)");
   return run_vae(m, xin, N, hw, out, workspace, workspace_bytes, stream, "vae_encode");
+}
+
+int bg_vae_encode_moments(BgVae* m, const float* xin, int N, int hw, float* moments, void* workspace, size_t workspace_bytes,
+                          void* stream) {
+  BG_REQUIRE(m && xin && moments && workspace && N > 0, "vae_encode_moments: bad arguments");
+  BG_REQUIRE(m->kind == 2 || m->kind == 3, "vae_encode_moments: handle is not an encoder");
+  BG_REQUIRE(m->kind == 2 ? (hw == 8 || hw == 16 || hw == 24 || hw == 32) : hw == 32,
+             "vae_encode_moments: input extent must be 8/16/24/32 (surface) or 32 (edge)");
+  Tail t;
+  t.moments = moments;
+  return run_vae(m, xin, N, hw, nullptr, workspace, workspace_bytes, stream, "vae_encode_moments", &t);
+}
+
+int bg_vae_posterior(const float* moments, const float* noise, int N, int P, int deterministic, float* z, float* kl,
+                     void* stream) {
+  BG_TRY(bg_check_device());
+  BG_REQUIRE(moments && N > 0 && P > 0, "vae_posterior: bad arguments");
+  Tail t;
+  t.noise = noise;
+  t.z = z;
+  t.kl = kl;
+  return posterior(op_ctx(N, stream), nullptr, 0, nullptr, nullptr, moments, t, P, deterministic);
+}
+
+// The round trip shares one carve between the encoder and then the decoder; z follows it, outside the carve.
+static size_t recon_carve_bytes(const BgVae* enc, const BgVae* dec, size_t N) {
+  return std::max(carve_vae(nullptr, enc->kind, N).bytes, carve_vae(nullptr, dec->kind, N).bytes);
+}
+
+size_t bg_vae_reconstruct_workspace_bytes(const BgVae* enc, const BgVae* dec, int N) {
+  if (!enc || !dec || N <= 0) return 0;
+  const size_t max_p = enc->kind == 2 ? 16 : 4;      // latent positions at the largest extent (32 x 32 / 32 points)
+  return recon_carve_bytes(enc, dec, (size_t)N) + align_up((size_t)N * 3 * max_p * 4, 1024) + 1024;
+}
+
+int bg_vae_reconstruct(BgVae* enc, BgVae* dec, const float* x, int N, int hw, const float* noise, float* moments, float* z,
+                       float* kl, float* dec_out, float* mse, void* workspace, size_t workspace_bytes, void* stream) {
+  BG_REQUIRE(enc && dec && x && dec_out && workspace && N > 0, "vae_reconstruct: bad arguments");
+  BG_REQUIRE((enc->kind == 2 || enc->kind == 3) && dec->kind == enc->kind - 2,
+             "vae_reconstruct: needs an encoder handle and the decoder handle of the same family");
+  BG_REQUIRE(enc->kind == 2 ? (hw == 8 || hw == 16 || hw == 24 || hw == 32) : hw == 32,
+             "vae_reconstruct: input extent must be 8/16/24/32 (surface) or 32 (edge)");
+  const int lat = hw / 8, P = enc->kind == 2 ? lat * lat : lat, vals = 3 * hw * (enc->kind == 2 ? hw : 1);
+  const size_t carve = recon_carve_bytes(enc, dec, (size_t)N);
+  char* base;
+  BG_TRY(align_workspace(workspace, workspace_bytes, carve + align_up((size_t)N * 3 * P * 4, 1024), "vae_reconstruct", &base));
+  Tail t;
+  t.noise = noise;
+  t.moments = moments;
+  t.kl = kl;
+  t.z = z ? z : reinterpret_cast<float*>(base + carve);
+  BG_TRY(run_vae(enc, x, N, hw, nullptr, base, carve, stream, "vae_reconstruct", &t));
+  BG_TRY(run_vae(dec, t.z, N, lat, dec_out, base, carve, stream, "vae_reconstruct"));
+  return mse ? sample_mse(op_ctx(N, stream), dec_out, x, vals, mse) : BG_OK;
 }
 
 // ---- unit-level entry points: the networks' own launch code on caller-owned buffers

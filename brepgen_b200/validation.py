@@ -7,6 +7,9 @@ Host glue only: `model`, `surf_vae`, `edge_vae` and `noise_scheduler` are the dr
 vae.py, schedulers.py) -- or any callables with the reference's signatures -- and carry the CUDA work.  The random draws
 follow the reference statement by statement (timesteps with torch.randint on the data's device, noise with torch.randn on
 the CPU generator and then moved), so a seeded run reproduces the reference's numbers (tests/golden/val_golden.npz).
+The two VAE trainers' `test_val()` loop bodies (trainer.py:116-124 surface, :246-254 edge: encode -> posterior sample ->
+decode -> per-sample MSE) are `surfvae_val_losses` / `edgevae_val_losses`, and `vae_val_mse` is their loop
+(tests/golden/vae_val_golden.npz).
 The training step itself (autograd, AdamW, GradScaler; trainer.py:497-541 etc.) is out of scope: the product is
 inference-only.
 """
@@ -94,3 +97,41 @@ def edgez_val_losses(model, surf_vae, edge_vae, noise_scheduler, edgePnt, edgePo
             pred = model(diffused, timesteps, edgePos, surfPos, surfZ, edge_mask, class_label)
         out.append(_mse_rows(pred[~edge_mask], noise[~edge_mask]))
     return out
+
+
+def _vae_val_loss(model, x: torch.Tensor, rng_device=None) -> float:
+    """encode -> posterior.sample() -> decode -> per-sample MSE summed over the batch.  The drop-in auto-encoders run it as
+    one fused round trip (`reconstruct`); any other model with the reference's encode / decode surface runs the statements
+    one by one.  rng_device="cpu" draws the posterior noise on the CPU generator (see _draw)."""
+    generator = torch.default_generator if rng_device == "cpu" else None
+    with torch.no_grad():
+        if hasattr(model, "reconstruct"):
+            return float(model.reconstruct(x, sample_posterior=True, generator=generator)[1].sum().item())
+        posterior = model.encode(x).latent_dist
+        z = posterior.sample(generator=generator)
+        dec = model.decode(z).sample
+        return float(((dec - x) ** 2).mean(tuple(range(1, x.dim()))).sum().item())
+
+
+def surfvae_val_losses(model, surf_uv: torch.Tensor, rng_device=None) -> float:
+    """SurfVAETrainer.test_val loop body (trainer.py:116-124): surf_uv (N, 32, 32, 3) as the dataloader yields it -> the
+    sum over the batch of the per-sample reconstruction MSE, the posterior sampled as the reference samples it"""
+    return _vae_val_loss(model, surf_uv.permute(0, 3, 1, 2), rng_device)
+
+
+def edgevae_val_losses(model, edge_u: torch.Tensor, rng_device=None) -> float:
+    """EdgeVAETrainer.test_val loop body (trainer.py:246-254): edge_u (N, 32, 3) -> summed per-sample MSE"""
+    return _vae_val_loss(model, edge_u.permute(0, 2, 1), rng_device)
+
+
+def vae_val_mse(model, batches, edge: bool = False, device=None, rng_device=None) -> float:
+    """SurfVAETrainer / EdgeVAETrainer.test_val (trainer.py:106-129, :236-259): total_loss / total_count over the batches of
+    a validation loader"""
+    fn = edgevae_val_losses if edge else surfvae_val_losses
+    total_loss, total_count = 0.0, 0
+    for batch in batches:
+        if device is not None:
+            batch = batch.to(device)
+        total_loss += fn(model, batch, rng_device)
+        total_count += len(batch)
+    return total_loss / total_count

@@ -96,6 +96,9 @@ int bg_denoiser_forward(BgDenoiser* m, const BgDenoiserArgs* args, void* workspa
 typedef struct BgVae BgVae;
 /* kind: 0 surface decoder, 1 edge decoder, 2 surface encoder, 3 edge encoder */
 int bg_vae_create(int kind, const BgNamedTensor* weights, int n_weights, void* stream, BgVae** out);
+/* bg_vae_create with the number of product terms of the compensated fp16 GEMMs: 0 = the default of the kind (3; 2 for the
+ * edge decoder), 3 = A_hi W_hi + A_lo W_hi + A_hi W_lo, 2 = A_hi W_hi + A_hi W_lo (a third less GEMM work, larger error) */
+int bg_vae_create_ex(int kind, int terms, const BgNamedTensor* weights, int n_weights, void* stream, BgVae** out);
 void bg_vae_destroy(BgVae* m);
 size_t bg_vae_workspace_bytes(const BgVae* m, int N);
 int bg_vae_decode(BgVae* m, const float* z, int N, float* out, void* workspace, size_t workspace_bytes, void* stream);
@@ -107,6 +110,27 @@ int bg_vae_decode_hw(BgVae* m, const float* z, int N, int hw, float* out, void* 
  * network.py:745-783, x (N,3,32) -> (N,3,4).  `weights`: `encoder.*` and `quant_conv.*`. */
 int bg_vae_encode(BgVae* m, const float* x, int N, int hw, float* out, void* workspace, size_t workspace_bytes,
                   void* stream);
+/* The full auto-encoders (diffusers AutoencoderKL, trainer.py:20-30, and the reference's AutoencoderKL1D, network.py:316-687):
+ * the encoder's posterior, diffusers' DiagonalGaussianDistribution over moments = quant_conv(encoder(x)), P latent positions
+ * per sample (hw/8 x hw/8 surface, 4 edge).
+ * encode_moments: kind 2 / 3 handle, x as bg_vae_encode -> moments (N,6,P) fp32, raw, mean = channels 0-2, logvar = 3-5;
+ *                 the mean half equals bg_vae_encode's output bit for bit.  Workspace: bg_vae_workspace_bytes.
+ * posterior:      caller moments (N,6,P) -> z (N,3,P) = mean + exp(0.5 clamp(logvar, -30, 20)) * noise (noise (N,3,P),
+ *                 NULL: z = mean) and kl (N) = 0.5 sum_{c,p} (mean^2 + var - 1 - logvar), var = exp(clamped logvar), summed
+ *                 in a fixed order (deterministic).  deterministic != 0: std = var = 0, so z = mean and kl = 0.  z / kl may
+ *                 be NULL.
+ * reconstruct:    encoder -> posterior -> decoder -> per-sample MSE in one stream-ordered call (no host synchronisation,
+ *                 graph-capturable): enc a kind 2 / 3 handle, dec the decoder of the same family (kind enc - 2), x (N,3,hw,hw)
+ *                 with hw in {8,16,24,32} or (N,3,32); dec_out has the shape of x; mse (N) = mean over C*H*W of
+ *                 (dec_out - x)^2.  noise, moments, z, kl, mse may be NULL (noise NULL: the decoder reads the mode).
+ *                 Workspace: bg_vae_reconstruct_workspace_bytes(enc, dec, N). */
+int bg_vae_encode_moments(BgVae* m, const float* x, int N, int hw, float* moments, void* workspace, size_t workspace_bytes,
+                          void* stream);
+int bg_vae_posterior(const float* moments, const float* noise, int N, int P, int deterministic, float* z, float* kl,
+                     void* stream);
+size_t bg_vae_reconstruct_workspace_bytes(const BgVae* enc, const BgVae* dec, int N);
+int bg_vae_reconstruct(BgVae* enc, BgVae* dec, const float* x, int N, int hw, const float* noise, float* moments, float* z,
+                       float* kl, float* dec_out, float* mse, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Scheduler updates.  Replace diffusers DDPMScheduler.step / PNDMScheduler.step as called at

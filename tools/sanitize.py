@@ -51,6 +51,13 @@ if what == "all":
     run("surface decoder", V.test_surface_decoder, 5, 2)
     run("edge decoder", V.test_edge_decoder, 37, 16)
     run("encoders", V.test_encoders_match_oracle)
+    import test_gpu_vae_posterior as VP
+    run("posterior tail", VP.test_moments_match_oracle_and_mean_equals_encode, "surf", 24)
+    run("posterior tail", VP.test_moments_match_oracle_and_mean_equals_encode, "edge", 32)
+    run("reconstruct", VP.test_posterior_z_kl_mse_match_fp64, "surf")
+    run("reconstruct", VP.test_reconstruct_equals_unfused_entry_points, "edge")
+    run("reconstruct graph", VP.test_graph_replayed_chunks_equal_eager, "edge", 29, 8)
+    run("reconstruct bad args", VP.test_bad_arguments_are_reported_not_faulted)
     run("post topology", P.test_topology_and_edges_match_reference, list(P.CASES)[0])
     run("post joint optimize", P.test_joint_optimize_matches_reference, list(P.CASES)[0])
 print("SANITIZE_DONE", flush=True)
