@@ -5,21 +5,29 @@
 // Edge stages run ONE sequence of L = faces*edges <= 4000 tokens per sample (network.py:1265-1283), so this is an
 // online-softmax (flash) kernel; the surface stages (L <= 100) use the same kernel with one key block.
 //
-// CTA = one 128-row query tile of one (sample, head), 384 threads = 3 warpgroups:
-//   warpgroup 0    : TMA producer (one elected thread: Q once; K / V 128-key tiles through an ST-deep mbarrier ring);
-//                    gives its registers to the consumers (setmaxnreg)
-//   warpgroups 1-2 : consumers, 64 query rows each; per key block j:
+// CTA = one 192-row query tile of one (sample, head), 512 threads = 4 warpgroups:
+//   warpgroup 0    : TMA producer (one elected thread: Q once; K / V 128-key tiles through an ST-deep mbarrier ring)
+//   warpgroups 1-3 : consumers, 64 query rows each; per key block j:
 //                      S = Q K_j^T          4 x wgmma m64n128k16, Q and K K-major SW128 from shared memory
 //                      P = exp2(c (S - m))  in registers (fp32 online softmax, rows split over lane quads)
 //                      O = O a + P V_j      8 x wgmma m64n64k16, A = P as fp16 straight from the S registers,
 //                                           B = V MN-major SW128 from shared memory
-//                    S, P and O never leave the registers; the two consumer warpgroups interleave on the tensor core.
-// The exponentials cost about as many SM clocks as the MMAs at head dim 64, so within a warpgroup the two overlap:
-// S_{j+1} = Q K_{j+1}^T and O += P_j V_j are issued together, and the softmax of block j + 1 runs while P_j V_j is still
-// on the tensor core (registers for S_{j+1} and the fp16 P_j at once).  Handing the tensor core between the two
-// warpgroups in strict turns (named barriers) measured slower than leaving them to interleave, and is not done.
-// The arithmetic (MMA sequence, max / alpha / exp2 / row-sum order, O *= alpha before O += P V) is that of a plain
-// block-by-block loop: the pipelining changes when instructions run, not what they compute.
+//                    S, P and O never leave the registers.
+// The exponentials cost about as many SM clocks as the MMAs at head dim 64, so the tensor core and the MUFU unit must
+// work at the same time.  Three consumer warpgroups are three independent instruction streams, one warp each per SM
+// sub-partition: while one warpgroup runs its softmax, the others keep the tensor core busy.  Each warpgroup runs a plain
+// block loop (S_j, softmax, O += P_j V_j, then block j + 1).  Issuing S_{j+1} together with P_j V_j, as the two-consumer
+// 128-row kernel did, pins S_{j+1}, the fp16 P_j and O at once (128 registers), and 512 threads leave 128 registers per
+// thread: ptxas allocates within that launch bound whatever setmaxnreg grants later, and that form spills.  The plain
+// loop fits without spills and measured faster than the pipelined 128-row kernel (DESIGN.md §5).  The producer still
+// drops to 24 registers and the consumers ask for 160 (128 * 24 + 384 * 160 <= 64 K): the same code without the
+// setmaxnreg pair measured 1.05x instead of 1.11-1.15x over the 128-row kernel.
+// The wider tile also wastes less at the sequence end (L = 4000: last tile 160 of 192 rows, against 32 of 128) and reads
+// each K / V tile for 192 query rows instead of 128.
+// A consumer warpgroup whose 64 rows all lie at or past the sample's length skips the key loop; the ring's empty
+// barriers count one arrival per warp of the warpgroups that take part.
+// The arithmetic (MMA sequence, max / alpha / exp2 / row-sum order, O *= alpha before O += P V) depends only on the row
+// and the order of the key blocks, not on the tile height: the outputs are those of the 128-row kernels bit for bit.
 // Fully padded key blocks are skipped through a per-sample block list (result-preserving: their p is exactly 0).
 // Roofline: tensor-bound; 4*L*L*64 flop per (sample, head).
 #include <math.h>
@@ -35,18 +43,20 @@ namespace {
 constexpr int DH = 64;
 constexpr int NHEAD = 12;
 constexpr int DMODEL = 768;
-constexpr int BQ = 128;                    // query rows per CTA (two consumer warpgroups of 64)
-constexpr int TILE_BYTES = 128 * DH * 2;   // 16 KB: Q / K / V tile, 128 rows x 128 B
-constexpr int ST = 2;                      // K / V ring depth (4 measured no faster)
+constexpr int NCW = 3;                     // consumer warpgroups, 64 query rows each
+constexpr int BQ = NCW * 64;               // 192 query rows per CTA
+constexpr int Q_BYTES = BQ * DH * 2;       // 24 KB: Q tile, 192 rows x 128 B
+constexpr int TILE_BYTES = 128 * DH * 2;   // 16 KB: K / V tile, 128 rows x 128 B
+constexpr int ST = 4;                      // K / V ring depth: lets the three consumer warpgroups drift apart
 constexpr int OFF_Q = 0;
-constexpr int OFF_K = TILE_BYTES;
+constexpr int OFF_K = Q_BYTES;
 constexpr int OFF_V = OFF_K + ST * TILE_BYTES;
 constexpr int OFF_BAR = OFF_V + ST * TILE_BYTES;
 constexpr int OFF_MASKW = OFF_BAR + 256;   // invalid-key bit words: 4 per key block, MAX_KB blocks
 constexpr int MAX_KB = ATTN_MAX_L / 128;   // 64 key blocks: L <= 8192
 constexpr int SMEM_BYTES = OFF_MASKW + MAX_KB * 16 + 1024;
-constexpr int THREADS = 384;
-constexpr int CONSUMER_THREADS = 256;
+constexpr int THREADS = 128 * (NCW + 1);
+static_assert(OFF_K % 1024 == 0, "K / V tiles must start on 1024-byte boundaries (SW128)");
 
 struct AttnParams {
   __half* out;
@@ -160,7 +170,7 @@ __device__ __forceinline__ void pack_p(uint32_t (&pa)[8][4], const float (&sc)[6
 }
 
 __global__ void __launch_bounds__(THREADS, 1)
-attn_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParams p) {
+attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV, const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
@@ -183,15 +193,19 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParams p) {
   if (qgrp * BQ >= len) return;     // variable-length mode: the grid is sized for the longest sample
   const int nblk = p.blk_count ? p.blk_count[b] : (len + 127) / 128;
   const int* blist = p.blk_list ? p.blk_list + (size_t)b * p.nkb : nullptr;
+  // consumer warpgroups with at least one query row < len (1..NCW); the others skip the key loop, so the empty barriers
+  // count only the arrivals of these, one per warp
+  const int nact = min(NCW, (len - qgrp * BQ + 63) / 64);
 
   if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmQKV);
+    tma_prefetch_desc(&tmQ);
+    tma_prefetch_desc(&tmKV);
     mbar_init(q_full, 1);
     for (int i = 0; i < ST; ++i) {
       mbar_init(&k_full[i], 1);
-      mbar_init(&k_empty[i], CONSUMER_THREADS);
+      mbar_init(&k_empty[i], nact * 4);
       mbar_init(&v_full[i], 1);
-      mbar_init(&v_empty[i], CONSUMER_THREADS);
+      mbar_init(&v_empty[i], nact * 4);
     }
     fence_barrier_init();
   }
@@ -226,103 +240,68 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParams p) {
   if (wg == 0) {
     setmaxnreg_dec<24>();
     if (warp == 0 && elect_one()) {
-      mbar_arrive_expect_tx(q_full, TILE_BYTES);
-      tma_load_2d(smem + OFF_Q, &tmQKV, q_full, h * DH, row0 + qgrp * BQ);
+      mbar_arrive_expect_tx(q_full, Q_BYTES);
+      tma_load_2d(smem + OFF_Q, &tmQ, q_full, h * DH, row0 + qgrp * BQ);
       Ring r;
       for (int it = 0; it < nblk; ++it, r.advance()) {
         const int kb = blist ? blist[it] : it;
         const int s = r.stage;
         mbar_wait(&k_empty[s], r.phase ^ 1u);
         mbar_arrive_expect_tx(&k_full[s], TILE_BYTES);
-        tma_load_2d(smem + OFF_K + s * TILE_BYTES, &tmQKV, &k_full[s], DMODEL + h * DH, row0 + kb * 128);
+        tma_load_2d(smem + OFF_K + s * TILE_BYTES, &tmKV, &k_full[s], DMODEL + h * DH, row0 + kb * 128);
         mbar_wait(&v_empty[s], r.phase ^ 1u);
         mbar_arrive_expect_tx(&v_full[s], TILE_BYTES);
-        tma_load_2d(smem + OFF_V + s * TILE_BYTES, &tmQKV, &v_full[s], 2 * DMODEL + h * DH, row0 + kb * 128);
+        tma_load_2d(smem + OFF_V + s * TILE_BYTES, &tmKV, &v_full[s], 2 * DMODEL + h * DH, row0 + kb * 128);
       }
     }
     return;
   }
 
-  setmaxnreg_inc<240>();
+  const int cw = wg - 1;             // consumer warpgroup index: query rows [64 cw, 64 cw + 64) of the tile
+  if (cw >= nact) return;            // all its rows are >= len
+  setmaxnreg_inc<160>();
   // ------------------------------------------------------------------ consumer warpgroup: 64 query rows
   // Accumulator layout (wgmma m64nN, fp32): warp w of the warpgroup owns rows 16w + lane / 4 (elements 4i, 4i + 1) and
   // 16w + 8 + lane / 4 (elements 4i + 2, 4i + 3), at columns 8i + 2 (lane % 4) + {0, 1}.  Every row is spread over one
   // lane quad, so row statistics need two shuffles.
-  const int half = wg - 1;
   const int wq = warp & 3;
   const float c = p.scale_log2;
-  const uint32_t q_addr = smem_u32(smem + OFF_Q) + half * 64 * 128;
+  const uint32_t q_addr = smem_u32(smem + OFF_Q) + cw * 64 * 128;
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
   float o[DH / 2];
 #pragma unroll
   for (int i = 0; i < DH / 2; ++i) o[i] = 0.f;
 
   mbar_wait(q_full, 0);
-  if (nblk > 0) {
-    const uint32_t k_base = smem_u32(smem + OFF_K), v_base = smem_u32(smem + OFF_V);
-    Ring kr, vr;                 // K_j is consumed in step j, V_j one step later
+  const uint32_t k_base = smem_u32(smem + OFF_K), v_base = smem_u32(smem + OFF_V);
+  Ring r;
+#pragma unroll 1
+  for (int it = 0; it < nblk; ++it, r.advance()) {
     float sc[64], alpha[2];
     uint32_t pa[8][4];
-
-    // step 0: S_0 alone
-    mbar_wait(&k_full[kr.stage], kr.phase);
+    mbar_wait(&k_full[r.stage], r.phase);
     wgmma_fence();
-    issue_qk(sc, q_addr, k_base + kr.stage * TILE_BYTES);
+    issue_qk(sc, q_addr, k_base + r.stage * TILE_BYTES);
     wgmma_wait<0>();
     wgmma_fence_operand(sc);
-    mbar_arrive(&k_empty[kr.stage]);
-    kr.advance();
-    softmax_block(sc, maskw, m_run, l_run, alpha, c, lane);
-
-    // step j: S_j and O += P_{j-1} V_{j-1} on the tensor core; the softmax of S_j runs while P_{j-1} V_{j-1} finishes.
-    // The wait for P_{j-1} V_{j-1} sits at the top of the next step: within one step the compiler would schedule the
-    // exponentials below it, and nothing would overlap.
-#pragma unroll 1
-    for (int it = 1; it < nblk; ++it) {
-      wgmma_wait<0>();
-      wgmma_fence_operand(o);
-      if (it >= 2) {             // P_{it-2} V_{it-2} has finished with its V stage
-        mbar_arrive(&v_empty[vr.stage]);
-        vr.advance();
-      }
-      scale_o(o, alpha);
-      pack_p(pa, sc);
-      mbar_wait(&k_full[kr.stage], kr.phase);
-      mbar_wait(&v_full[vr.stage], vr.phase);
-      wgmma_fence_operand(o);
-      wgmma_fence();
-      issue_qk(sc, q_addr, k_base + kr.stage * TILE_BYTES);
-      issue_pv(o, pa, v_base + vr.stage * TILE_BYTES);
-      wgmma_wait<1>();
-      wgmma_fence_operand(sc);
-      mbar_arrive(&k_empty[kr.stage]);
-      kr.advance();
-      softmax_block(sc, maskw + it * 4, m_run, l_run, alpha, c, lane);
-    }
-
-    // step nblk: O += P_{nblk-1} V_{nblk-1}
-    wgmma_wait<0>();
-    wgmma_fence_operand(o);
-    if (nblk >= 2) {
-      mbar_arrive(&v_empty[vr.stage]);
-      vr.advance();
-    }
+    if (lane == 0) mbar_arrive(&k_empty[r.stage]);   // the warp is past its wait: its MMAs are done with the stage
+    softmax_block(sc, maskw + it * 4, m_run, l_run, alpha, c, lane);
     scale_o(o, alpha);
     pack_p(pa, sc);
-    mbar_wait(&v_full[vr.stage], vr.phase);
+    mbar_wait(&v_full[r.stage], r.phase);
     wgmma_fence_operand(o);
     wgmma_fence();
-    issue_pv(o, pa, v_base + vr.stage * TILE_BYTES);
+    issue_pv(o, pa, v_base + r.stage * TILE_BYTES);
     wgmma_wait<0>();
     wgmma_fence_operand(o);
-    mbar_arrive(&v_empty[vr.stage]);
+    if (lane == 0) mbar_arrive(&v_empty[r.stage]);
   }
 
 #pragma unroll
   for (int hr = 0; hr < 2; ++hr) {
     const float l = quad_sum(l_run[hr]);
     const float inv = l > 0.f ? 1.f / l : 0.f;
-    const int row = qgrp * BQ + half * 64 + wq * 16 + hr * 8 + (lane >> 2);
+    const int row = qgrp * BQ + cw * 64 + wq * 16 + hr * 8 + (lane >> 2);
     if (row >= len) continue;
     __half* dst = p.out + ((size_t)row0 + row) * p.ldo + h * DH + 2 * (lane & 3);
 #pragma unroll
@@ -376,10 +355,11 @@ int launch_attention(cudaStream_t st, const AttnArgs& a) {
   BG_REQUIRE(a.ldo % 8 == 0, "attention: output pitch must be a multiple of 8");
   BG_REQUIRE(a.L <= ATTN_MAX_L, "attention: sequence longer than 8192 tokens is not supported");
   BG_REQUIRE((a.blk_list == nullptr) == (a.blk_count == nullptr), "attention: blk_list and blk_count go together");
-  CUtensorMap tm;
+  CUtensorMap tmQ, tmKV;
   BG_REQUIRE((a.seq_row0 == nullptr) == (a.seq_len == nullptr), "attention: seq_row0 and seq_len go together");
   BG_REQUIRE(a.seq_len == nullptr || (a.key_mask == nullptr && a.blk_list == nullptr), "attention: variable-length mode takes no mask");
-  BG_TRY(make_tmap_2d_f16(&tm, a.qkv, (uint64_t)a.B * (uint64_t)a.L, 3 * DMODEL, 3 * DMODEL, 128));
+  BG_TRY(make_tmap_2d_f16(&tmQ, a.qkv, (uint64_t)a.B * (uint64_t)a.L, 3 * DMODEL, 3 * DMODEL, BQ));
+  BG_TRY(make_tmap_2d_f16(&tmKV, a.qkv, (uint64_t)a.B * (uint64_t)a.L, 3 * DMODEL, 3 * DMODEL, 128));
   AttnParams p;
   p.out = a.out; p.ldo = a.ldo; p.B = a.B; p.L = a.L; p.nkb = (a.L + 127) / 128;
   p.key_mask = a.key_mask; p.blk_list = a.blk_list; p.blk_count = a.blk_count; p.blk_words = a.blk_words;
@@ -387,7 +367,7 @@ int launch_attention(cudaStream_t st, const AttnArgs& a) {
   p.scale_log2 = 1.4426950408889634f / 8.0f;
   BG_TRY(ensure_dynamic_smem(reinterpret_cast<const void*>(&attn_kernel), SMEM_BYTES));
   dim3 grid((a.L + BQ - 1) / BQ, NHEAD, a.B);
-  attn_kernel<<<grid, THREADS, SMEM_BYTES, st>>>(tm, p);
+  attn_kernel<<<grid, THREADS, SMEM_BYTES, st>>>(tmQ, tmKV, p);
   return check_launch("attn_kernel launch");
 }
 
