@@ -112,6 +112,85 @@ __global__ void __launch_bounds__(256) ddpm_step_tab_kernel(const DdpmTabP p) {
     }
   }
 }
+// Per-sample noise streams: element j of sample b is normal (j % 4) of Philox4x32-10 with key keys[b] and counter
+// (j / 4 as 64 bits, t, domain); domain 0 = DDPM step noise at timestep t, 1 = initial noise (t = 0).  A group of 4 never
+// straddles two samples (the last group of a sample uses its first per_sample % 4 normals), so a sample's noise does not
+// depend on the batch it sits in, on its position there, or on the rank that runs it.
+__device__ __forceinline__ void keyed_normal4(unsigned long long key, unsigned long long q, uint32_t t, uint32_t domain,
+                                              float (&z)[4]) {
+  uint32_t r[4];
+  philox4x32_10((uint32_t)q, (uint32_t)(q >> 32), t, domain, (uint32_t)key, (uint32_t)(key >> 32), r);
+  box_muller(r[0], r[1], z[0], z[1]);
+  box_muller(r[2], r[3], z[2], z[3]);
+}
+
+struct RandnKeyedP {
+  const unsigned long long* keys;
+  float* out;
+  long long n_samples, per_sample;
+  uint32_t domain, t;
+};
+__global__ void __launch_bounds__(256) randn_keyed_kernel(const RandnKeyedP p) {
+  const long long gps = (p.per_sample + 3) / 4, ng = p.n_samples * gps;
+  for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += (long long)gridDim.x * blockDim.x) {
+    const long long b = g / gps, q = g - b * gps;
+    float z[4];
+    keyed_normal4(p.keys[b], (unsigned long long)q, p.t, p.domain, z);
+    float* o = p.out + b * p.per_sample;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const long long i = q * 4 + j;
+      if (i >= p.per_sample) break;
+      o[i] = z[j];
+    }
+  }
+}
+
+// The DDPM update of ddpm_step_kernel with per-sample noise: the expressions are written exactly as there, so the keyed
+// step with noise == NULL is bit-identical to bg_ddpm_step fed the tensor bg_randn_keyed(domain 0, t) writes.
+// Table form (coef != NULL): coefficients from coef[*step], timestep from *t_cur, as ddpm_step_tab_kernel.
+struct DdpmKeyedP {
+  const float *eps_c, *eps_u, *x, *noise;
+  float* out;
+  long long n, per_sample;
+  float w, sb, sa, clip, c_x0, c_x, sigma;
+  const unsigned long long* keys;
+  long long t;
+  const float* coef;
+  const int* step;
+  const long long* t_cur;
+};
+__global__ void __launch_bounds__(256) ddpm_step_keyed_kernel(const DdpmKeyedP p) {
+  float sb = p.sb, sa = p.sa, c_x0 = p.c_x0, c_x = p.c_x, sigma = p.sigma;
+  long long t = p.t;
+  if (p.coef) {
+    const float* cf = p.coef + 5 * (long long)*p.step;
+    sb = cf[0]; sa = cf[1]; c_x0 = cf[2]; c_x = cf[3]; sigma = cf[4];
+    t = *p.t_cur;
+  }
+  const long long gps = (p.per_sample + 3) / 4, ng = (p.n / p.per_sample) * gps;
+  for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += (long long)gridDim.x * blockDim.x) {
+    const long long b = g / gps, q = g - b * gps;
+    float z[4] = {0.f, 0.f, 0.f, 0.f};
+    if (sigma != 0.f && p.noise == nullptr) keyed_normal4(p.keys[b], (unsigned long long)q, (uint32_t)t, 0u, z);
+    const long long base = b * p.per_sample;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const long long js = q * 4 + j;
+      if (js >= p.per_sample) break;
+      const long long i = base + js;
+      float e = p.eps_c[i];
+      if (p.eps_u) e = e * (1.f + p.w) - p.eps_u[i] * p.w;
+      const float xv = p.x[i];
+      float x0 = (xv - sb * e) / sa;
+      if (p.clip > 0.f) x0 = fminf(fmaxf(x0, -p.clip), p.clip);
+      float o = c_x0 * x0 + c_x * xv;
+      if (sigma != 0.f) o += sigma * (p.noise ? p.noise[i] : z[j]);
+      p.out[i] = o;
+    }
+  }
+}
+
 // one thread: k = ++(*step);  *t_cur = ts[k]   (the denoiser reads its timestep from t_cur, the step kernel reads k)
 __global__ void step_advance_kernel(const long long* __restrict__ ts, int n, int* __restrict__ step, long long* __restrict__ t_cur) {
   int k = *step + 1;
@@ -179,6 +258,51 @@ int bg_ddpm_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w
   p.coef = coef_table; p.step = step; p.seed = seed; p.offset0 = offset0; p.offset_stride = offset_stride;
   ddpm_step_tab_kernel<<<grid_for((n + 3) / 4), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
   return check_launch("ddpm_step_tab_kernel launch");
+}
+
+int bg_randn_keyed(const uint64_t* sample_keys, int64_t n_samples, int64_t per_sample, int32_t domain, int64_t t, float* out,
+                   void* stream) {
+  BG_REQUIRE(sample_keys && out, "randn_keyed: sample_keys and out must not be NULL");
+  BG_REQUIRE(n_samples > 0 && per_sample > 0, "randn_keyed: n_samples and per_sample must be positive");
+  BG_REQUIRE(domain >= 0 && t >= 0 && t <= 0xFFFFFFFFll, "randn_keyed: domain and t must be 32-bit unsigned values");
+  RandnKeyedP p;
+  p.keys = reinterpret_cast<const unsigned long long*>(sample_keys); p.out = out;
+  p.n_samples = n_samples; p.per_sample = per_sample; p.domain = (uint32_t)domain; p.t = (uint32_t)t;
+  randn_keyed_kernel<<<grid_for(n_samples * ((per_sample + 3) / 4)), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch("randn_keyed_kernel launch");
+}
+
+int bg_ddpm_step_keyed(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
+                       const float* noise, const uint64_t* sample_keys, int64_t per_sample, int64_t t, int64_t n,
+                       float sqrt_one_minus_abar, float sqrt_abar, float clip, float c_x0, float c_x, float sigma,
+                       void* stream) {
+  BG_REQUIRE(eps_cond && x && out && n > 0, "ddpm_step_keyed: bad arguments");
+  BG_REQUIRE(sample_keys != nullptr, "ddpm_step_keyed: sample_keys must not be NULL");
+  BG_REQUIRE(per_sample > 0 && n % per_sample == 0, "ddpm_step_keyed: n must be a positive multiple of per_sample");
+  BG_REQUIRE(t >= 0 && t <= 0xFFFFFFFFll, "ddpm_step_keyed: t must be a 32-bit unsigned value");
+  BG_REQUIRE(sqrt_abar > 0.f, "ddpm_step_keyed: sqrt_abar must be positive");
+  DdpmKeyedP p = {};
+  p.eps_c = eps_cond; p.eps_u = eps_uncond; p.x = x; p.noise = noise; p.out = out; p.n = n; p.per_sample = per_sample;
+  p.w = cfg_w; p.sb = sqrt_one_minus_abar; p.sa = sqrt_abar; p.clip = clip; p.c_x0 = c_x0; p.c_x = c_x; p.sigma = sigma;
+  p.keys = reinterpret_cast<const unsigned long long*>(sample_keys); p.t = t;
+  ddpm_step_keyed_kernel<<<grid_for((n / per_sample) * ((per_sample + 3) / 4)), 256, 0,
+                           reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch("ddpm_step_keyed_kernel launch");
+}
+
+int bg_ddpm_step_tab_keyed(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
+                           const uint64_t* sample_keys, int64_t per_sample, const int64_t* t_cur, int64_t n,
+                           const float* coef_table, const int32_t* step, float clip, void* stream) {
+  BG_REQUIRE(eps_cond && x && out && n > 0 && coef_table && step && t_cur, "ddpm_step_tab_keyed: bad arguments");
+  BG_REQUIRE(sample_keys != nullptr, "ddpm_step_tab_keyed: sample_keys must not be NULL");
+  BG_REQUIRE(per_sample > 0 && n % per_sample == 0, "ddpm_step_tab_keyed: n must be a positive multiple of per_sample");
+  DdpmKeyedP p = {};
+  p.eps_c = eps_cond; p.eps_u = eps_uncond; p.x = x; p.out = out; p.n = n; p.per_sample = per_sample;
+  p.w = cfg_w; p.clip = clip; p.keys = reinterpret_cast<const unsigned long long*>(sample_keys);
+  p.coef = coef_table; p.step = step; p.t_cur = reinterpret_cast<const long long*>(t_cur);
+  ddpm_step_keyed_kernel<<<grid_for((n / per_sample) * ((per_sample + 3) / 4)), 256, 0,
+                           reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch("ddpm_step_keyed_kernel launch");
 }
 
 int bg_step_advance(const int64_t* timesteps, int n_steps, int32_t* step, int64_t* t_cur, void* stream) {

@@ -14,13 +14,15 @@ no collective on the hot path; `gather_outputs` is the one optional all_gather a
 """
 from __future__ import annotations
 
-from dataclasses import dataclass
-from typing import Dict, Optional
+from dataclasses import dataclass, replace
+from typing import Dict, List, Optional, Sequence
 
 import torch
 
 from . import _ffi
-from .schedulers import DDPMScheduler, PNDMScheduler
+from .schedulers import DDPMScheduler, PNDMScheduler, sample_keys, sample_seed
+
+NOISE_MODES = ("batch", "per_sample")
 
 TEXT2INT = {"uncond": 0, "bathtub": 1, "bed": 2, "bench": 3, "bookshelf": 4, "cabinet": 5, "chair": 6, "couch": 7,
             "lamp": 8, "sofa": 9, "table": 10}   # sample.py:21-32
@@ -44,6 +46,12 @@ class CascadeConfig:
     decode: bool = True
     graph: str = "auto"                  # "on" | "off" | "auto": capture each DDPM loop (advance, forward, fused step) in a CUDA
                                          # graph and replay it; auto = on for launch-bound shapes (few tokens, many steps)
+    noise: str = "batch"                 # "batch": initial noise from a CPU generator seeded with `seed` (the reference's
+                                         # draws), step noise from one Philox stream per (seed, rank, stage).  "per_sample":
+                                         # every sample has its own streams, keyed by its seed, so a B-rep is a function of
+                                         # (seed, global sample index) whatever the batch size or GPU count
+    sample_base: int = 0                 # per_sample: global index of this batch's first sample
+    sample_seeds: Optional[Sequence[int]] = None   # per_sample: one seed per sample instead of sample_seed(seed, index)
 
 
 def config_from_eval_args(eval_args: dict, **overrides) -> CascadeConfig:
@@ -96,6 +104,44 @@ def shard_batch(global_batch: int, rank: int, world_size: int):
     base, rem = divmod(global_batch, world_size)
     lo = rank * base + min(rank, rem)
     return lo, lo + base + (1 if rank < rem else 0)
+
+
+def shard_config(cfg: CascadeConfig, global_batch: int, rank: int, world_size: int) -> CascadeConfig:
+    """The per-sample-noise config of `rank`'s shard of a `global_batch`-sample run: batch_size and sample_base from
+    shard_batch (and its slice of cfg.sample_seeds).  N ranks running their shards generate the same B-reps as one GPU
+    running cfg with batch_size = global_batch."""
+    lo, hi = shard_batch(global_batch, rank, world_size)
+    seeds = None
+    if cfg.sample_seeds is not None:
+        if len(cfg.sample_seeds) != global_batch:
+            raise ValueError(f"sample_seeds has {len(cfg.sample_seeds)} entries for a batch of {global_batch}")
+        seeds = list(cfg.sample_seeds)[lo:hi]
+    return replace(cfg, noise="per_sample", batch_size=hi - lo, sample_base=cfg.sample_base + lo, sample_seeds=seeds)
+
+
+def per_sample_seeds(cfg: CascadeConfig) -> Optional[List[int]]:
+    """cfg's per-sample seeds (None in batch mode); raises on an unknown noise mode or a sample_seeds of the wrong length"""
+    if cfg.noise not in NOISE_MODES:
+        raise ValueError(f"CascadeConfig.noise must be one of {NOISE_MODES}, got {cfg.noise!r}")
+    if cfg.noise == "batch":
+        return None
+    if cfg.sample_seeds is not None:
+        if len(cfg.sample_seeds) != cfg.batch_size:
+            raise ValueError(f"sample_seeds has {len(cfg.sample_seeds)} entries for batch_size {cfg.batch_size}")
+        return [int(s) for s in cfg.sample_seeds]
+    return [sample_seed(int(cfg.seed), int(cfg.sample_base) + b) for b in range(cfg.batch_size)]
+
+
+def randn_keyed(seeds: Sequence[int], stage: int, shape, device, domain: int = 1, t: int = 0) -> torch.Tensor:
+    """(len(seeds), *shape[1:]) fp32 normals from the per-sample streams (bg_randn_keyed); default domain 1 = initial noise"""
+    B = len(seeds)
+    keys = torch.from_numpy(sample_keys(seeds, stage).view("int64")).to(device)
+    out = torch.empty((B,) + tuple(shape[1:]), dtype=torch.float32, device=device)
+    per = out[0].numel()
+    with torch.cuda.device(out.device):
+        _ffi.check(_ffi.lib().bg_randn_keyed(keys.data_ptr(), B, per, int(domain), int(t), out.data_ptr(),
+                                            _ffi.current_stream()), "bg_randn_keyed")
+    return out
 
 
 def dedup_surfaces(surfPos: torch.Tensor, threshold: float):
@@ -158,7 +204,11 @@ class Cascade:
         ts = timesteps.to(device=dev, dtype=torch.int64).contiguous()
         step = torch.full((1,), -1, dtype=torch.int32, device=dev)
         t_cur = torch.zeros(1, dtype=torch.int64, device=dev)
-        seed, off0, stride = self.ddpm.philox_stream(n)
+        keyed = self.ddpm.per_sample_noise
+        if keyed:     # per-sample streams counted by the device timestep t_cur: no offset to carry between graphs
+            keys = self.ddpm.sample_key_tensor(B, dev)
+        else:
+            seed, off0, stride = self.ddpm.philox_stream(n)
         clip = float(self.ddpm.config.clip_sample_range) if self.ddpm.config.clip_sample else 0.0
 
         def body():
@@ -167,6 +217,11 @@ class Cascade:
             pred = fwd(torch.cat([xb, xb], 0) if cfg.use_cf else xb, t_cur)
             pc = pred[:B] if cfg.use_cf else pred
             pu = pred[B:] if cfg.use_cf else None
+            if keyed:
+                _ffi.check(lib.bg_ddpm_step_tab_keyed(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(),
+                                                      xb.data_ptr(), keys.data_ptr(), n // B, t_cur.data_ptr(), n,
+                                                      coef.data_ptr(), step.data_ptr(), clip, st), "bg_ddpm_step_tab_keyed")
+                return
             _ffi.check(lib.bg_ddpm_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(), xb.data_ptr(),
                                             seed, off0, stride, n, coef.data_ptr(), step.data_ptr(), clip, st),
                        "bg_ddpm_step_tab")
@@ -188,7 +243,8 @@ class Cascade:
         for _ in range(T):
             g.replay()
         _ffi.note_replay(per_replay, T)
-        self.ddpm.advance_philox(n, T)
+        if not keyed:
+            self.ddpm.advance_philox(n, T)
         self.last_graph_steps = getattr(self, "last_graph_steps", 0) + T
         return xb
 
@@ -247,7 +303,11 @@ class Cascade:
     _STAGE_ID = {"surfPos": 0, "surfZ": 1, "edgePos": 2, "edgeZV": 3}
 
     def _stage(self, cfg, x, fwd, label2, gen, hybrid_ddpm_tail: bool, on_step=None, noise_fn=None, name="surfPos"):
-        self.ddpm.set_noise_seed(*getattr(self, "_noise_key", (int(cfg.seed), 0)), self._STAGE_ID[name])
+        seeds = getattr(self, "_sample_seeds", None)
+        if seeds is not None:
+            self.ddpm.set_sample_keys(sample_seeds=seeds, stage=self._STAGE_ID[name])
+        else:
+            self.ddpm.set_noise_seed(*getattr(self, "_noise_key", (int(cfg.seed), 0)), self._STAGE_ID[name])
         if cfg.schedule == "ddpm":
             self.ddpm.set_timesteps(cfg.ddpm_steps)
             return self._loop(cfg, self.ddpm, self.ddpm.timesteps, x, fwd, label2, gen, on_step, noise_fn)
@@ -266,7 +326,11 @@ class Cascade:
     @torch.no_grad()
     def run(self, cfg: CascadeConfig, init_noise: Optional[Dict[str, torch.Tensor]] = None, step_noise=None):
         """step_noise(stage_name, k, shape) -> tensor: explicit DDPM step noise (parity runs); default = in-kernel Philox
-        keyed by (cfg.seed, rank, stage): reproducible from cfg.seed, independent across ranks and stages."""
+        keyed by (cfg.seed, rank, stage): reproducible from cfg.seed, independent across ranks and stages.
+        cfg.noise == "per_sample": initial and step noise come from each sample's own streams (bg_randn_keyed and the keyed
+        step kernels), so sample b's outputs depend on its seed alone; init_noise / step_noise still take precedence."""
+        seeds = per_sample_seeds(cfg)
+        self._sample_seeds = seeds
         dev = self.device
         rank = 0
         try:
@@ -288,6 +352,8 @@ class Cascade:
         def noise(name, shape):
             if init_noise is not None and name in init_noise:
                 return init_noise[name].to(dev).float()
+            if seeds is not None:
+                return randn_keyed(seeds, self._STAGE_ID[name], shape, dev)
             return torch.randn(shape, generator=cpu_gen).to(dev)
 
         rep2 = (lambda t: torch.cat([t, t], 0)) if cfg.use_cf else (lambda t: t)

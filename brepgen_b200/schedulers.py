@@ -48,6 +48,29 @@ def mix_seed(*parts: int) -> int:
     return h
 
 
+def sample_seed(seed: int, index: int) -> int:
+    """64-bit seed of the sample at global index `index` of a run seeded with `seed` (per-sample noise mode).  A mix rather
+    than seed + index, so that runs with neighbouring seeds share no sample."""
+    return mix_seed(seed, index)
+
+
+def sample_keys(seeds, stage: int) -> np.ndarray:
+    """uint64 [len(seeds)]: the Philox key of each sample's noise streams in one cascade stage (bg_randn_keyed,
+    bg_ddpm_step_keyed)"""
+    return np.array([mix_seed(s, stage) for s in seeds], dtype=np.uint64)
+
+
+def randn_generators(shape, generators, device=None, dtype=torch.float32) -> torch.Tensor:
+    """diffusers' randn_tensor for a list of generators, one per batch element: element i of the batch is drawn from
+    generators[i] on the generators' device (CPU generators sample on the host) and the result is moved to `device`"""
+    shape = tuple(shape)
+    if len(generators) != shape[0]:
+        raise ValueError(f"got {len(generators)} generators for a batch of {shape[0]}")
+    gdev = generators[0].device if hasattr(generators[0], "device") else torch.device("cpu")
+    rows = [torch.randn((1,) + shape[1:], generator=g, device=gdev, dtype=dtype) for g in generators]
+    return torch.cat(rows, 0).to(device if device is not None else gdev)
+
+
 def _as_int(t) -> int:
     return int(t.item()) if torch.is_tensor(t) else int(t)
 
@@ -74,15 +97,45 @@ class DDPMScheduler:
         self.init_noise_sigma = 1.0
         self._philox_seed = None       # None: derived from torch.initial_seed() at first use (follows torch.manual_seed)
         self._philox_offset = 0
+        self._sample_seeds = None      # per-sample noise mode: None (batch-wide stream) or (seed, first, stage, seeds)
+        self._key_cache = {}
         self.set_timesteps(num_train_timesteps)
 
     def set_noise_seed(self, seed: int, *stream: int):
         """Key of the in-kernel Philox stream that `step` draws its noise from when neither `noise` nor `generator` is
         given: a 64-bit mix of `seed` and any further integers (rank, stage, ...).  Resets the stream offset, so a run is
         reproducible from the seed alone and different (seed, rank, stage) tuples give independent streams
-        (SURVEY.md 8(e): per-rank independent RNG streams)."""
+        (SURVEY.md 8(e): per-rank independent RNG streams).  Leaves per-sample mode."""
         self._philox_seed = mix_seed(seed, *stream)
         self._philox_offset = 0
+        self._sample_seeds = None
+
+    def set_sample_keys(self, seed: int = 0, first: int = 0, stage: int = 0, sample_seeds=None):
+        """Per-sample noise mode: sample i of the batch `step` is given draws its noise from its own Philox stream, keyed by
+        mix_seed(s_i, stage) and counted by (element // 4, t, 0), so its noise depends on neither the batch size nor its
+        position in the batch.  s_i = sample_seed(seed, first + i) (`first` = global index of the batch's first sample), or
+        sample_seeds[i] when given.  `noise=` and `generator=` still take precedence; set_noise_seed leaves this mode."""
+        self._sample_seeds = (int(seed), int(first), int(stage),
+                              None if sample_seeds is None else [int(s) for s in sample_seeds])
+        self._key_cache = {}
+
+    @property
+    def per_sample_noise(self) -> bool:
+        return self._sample_seeds is not None
+
+    def sample_key_tensor(self, batch: int, device) -> torch.Tensor:
+        """device int64 [batch] holding the uint64 keys of the per-sample mode set by set_sample_keys"""
+        if self._sample_seeds is None:
+            raise RuntimeError("DDPMScheduler: per-sample noise mode is not set (call set_sample_keys)")
+        seed, first, stage, seeds = self._sample_seeds
+        if seeds is None:
+            seeds = [sample_seed(seed, first + i) for i in range(batch)]
+        elif len(seeds) != batch:
+            raise ValueError(f"DDPMScheduler: {len(seeds)} sample seeds for a batch of {batch}")
+        key = (batch, str(device))
+        if key not in self._key_cache:
+            self._key_cache[key] = torch.from_numpy(sample_keys(seeds, stage).view(np.int64)).to(device)
+        return self._key_cache[key]
 
     def set_timesteps(self, num_inference_steps: int, device=None):
         n_train = self.config.num_train_timesteps
@@ -132,7 +185,10 @@ class DDPMScheduler:
              guidance_w: float = 0.0, out: Optional[torch.Tensor] = None):
         """x_{t-1}.  Extras over diffusers (all optional): `noise` = explicit N(0,1) tensor (parity runs),
         `model_output_uncond` + `guidance_w` = classifier-free combine fused into the step (sample.py:134),
-        `out` = destination (may be `sample` for an in-place update)."""
+        `out` = destination (may be `sample` for an in-place update).  `generator` may be one generator or, as in
+        diffusers, a list with one per batch element (sample i's noise from generator[i]; CPU generators sample on the
+        host).  Without `noise` or `generator` the noise comes from the in-kernel stream: batch-wide (set_noise_seed) or
+        per sample (set_sample_keys)."""
         # the C ABI takes raw pointers and one element count: every tensor must cover exactly sample.numel() elements
         for name, ten in (("model_output", model_output), ("model_output_uncond", model_output_uncond), ("noise", noise),
                           ("out", out)):
@@ -148,13 +204,27 @@ class DDPMScheduler:
         eps = model_output.float().contiguous()
         eps_u = None if model_output_uncond is None else model_output_uncond.float().contiguous()
         if noise is None and generator is not None and sigma != 0.0:
-            # diffusers' randn_tensor: a CPU generator samples on the CPU and the result is moved to the device
-            gdev = generator.device if hasattr(generator, "device") else torch.device("cpu")
-            noise = torch.randn(x.shape, generator=generator, device=x.device if gdev.type == "cuda" else "cpu",
-                                dtype=torch.float32)
+            if isinstance(generator, (list, tuple)):
+                # diffusers' randn_tensor with one generator per batch element (the reference's utils.py:62-97)
+                noise = randn_generators(x.shape, generator, x.device)
+            else:
+                # diffusers' randn_tensor: a CPU generator samples on the CPU and the result is moved to the device
+                gdev = generator.device if hasattr(generator, "device") else torch.device("cpu")
+                noise = torch.randn(x.shape, generator=generator, device=x.device if gdev.type == "cuda" else "cpu",
+                                    dtype=torch.float32)
         if noise is not None:
             noise = noise.to(device=x.device, dtype=torch.float32).contiguous()
         n = x.numel()
+        dst = torch.empty_like(x) if out is None else out
+        clip = float(self.config.clip_sample_range) if self.config.clip_sample else 0.0
+        if self._sample_seeds is not None:
+            keys = self.sample_key_tensor(x.shape[0], x.device)
+            with torch.cuda.device(x.device):
+                _ffi.check(_ffi.lib().bg_ddpm_step_keyed(eps.data_ptr(), _ffi.ptr(eps_u), float(guidance_w), x.data_ptr(),
+                                                        dst.data_ptr(), _ffi.ptr(noise), keys.data_ptr(), n // x.shape[0],
+                                                        t, n, sb, sa, clip, c_x0, c_x, sigma, _ffi.current_stream()),
+                           "bg_ddpm_step_keyed")
+            return SchedulerOutput(dst) if return_dict else (dst,)
         seed, offset = 0, 0
         if noise is None and sigma != 0.0:
             if self._philox_seed is None:
@@ -162,8 +232,6 @@ class DDPMScheduler:
             seed = self._philox_seed
             offset = self._philox_offset
             self._philox_offset += (n + 3) // 4
-        dst = torch.empty_like(x) if out is None else out
-        clip = float(self.config.clip_sample_range) if self.config.clip_sample else 0.0
         with torch.cuda.device(x.device):
             _ffi.check(_ffi.lib().bg_ddpm_step(eps.data_ptr(), _ffi.ptr(eps_u), float(guidance_w), x.data_ptr(),
                                               dst.data_ptr(), _ffi.ptr(noise), seed, offset, n, sb, sa, clip, c_x0, c_x,

@@ -153,6 +153,26 @@ int bg_ddpm_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w
 /* k = ++(*step) (clamped to n_steps - 1);  *t_cur = timesteps[k].  One tiny kernel at the top of every captured step: the
  * denoiser forward reads its timestep from t_cur (device int64), bg_ddpm_step_tab reads k. */
 int bg_step_advance(const int64_t* timesteps, int n_steps, int32_t* step, int64_t* t_cur, void* stream);
+/* Per-sample noise streams (opt-in; the functions above keep the batch-wide (seed, offset) stream).  sample_keys: device
+ * uint64 [n_samples], one Philox4x32-10 key per sample.  Element j of sample b is normal (j % 4) of the block with key
+ * sample_keys[b] and counter (j / 4 as 64 bits, t, domain), Box-Muller as bg_ddpm_step; a block of 4 never straddles two
+ * samples.  domain 0 = DDPM step noise at timestep t, domain 1 = initial noise (t = 0).  A sample's noise is therefore a
+ * function of its key alone, whatever the batch size, its position in the batch or the rank that runs it.
+ * NULL sample_keys, per_sample <= 0 or n not a multiple of per_sample: BG_STATUS_BAD_ARG, nothing is launched. */
+/* out[b * per_sample + j] = normal j of sample b  (n_samples * per_sample fp32) */
+int bg_randn_keyed(const uint64_t* sample_keys, int64_t n_samples, int64_t per_sample, int32_t domain, int64_t t, float* out,
+                   void* stream);
+/* bg_ddpm_step over n / per_sample samples of per_sample elements, noise from the per-sample streams at timestep t (domain 0)
+ * unless `noise` is given.  Bit-identical to bg_ddpm_step fed the tensor bg_randn_keyed(..., 0, t, ...) writes. */
+int bg_ddpm_step_keyed(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
+                       const float* noise, const uint64_t* sample_keys, int64_t per_sample, int64_t t, int64_t n,
+                       float sqrt_one_minus_abar, float sqrt_abar, float clip, float c_x0, float c_x, float sigma,
+                       void* stream);
+/* table-driven form for graph capture: coefficients from coef_table[*step] as bg_ddpm_step_tab, timestep t from the device
+ * int64 *t_cur that bg_step_advance writes; bit-identical to bg_ddpm_step_keyed at the same t. */
+int bg_ddpm_step_tab_keyed(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
+                           const uint64_t* sample_keys, int64_t per_sample, const int64_t* t_cur, int64_t n,
+                           const float* coef_table, const int32_t* step, float clip, void* stream);
 /* out = c_sample*x - c_eps*(w0*e0 + w1*e1 + w2*e2 + w3*e3)    (PNDM transfer + Adams-Bashforth / RK combination;
  * unused e_i may be NULL with w_i = 0) */
 int bg_pndm_step(const float* x, float* out, int64_t n, float c_sample, float c_eps, const float* e0, float w0,

@@ -34,6 +34,10 @@ run("attention", T.test_attention, 2, 257, "rand", 0)
 run("attention", T.test_attention, 2, 1000, "blocks", 1)
 run("layernorm", T.test_layernorm, 77, 0)
 run("scheduler steps", T.test_ddpm_and_pndm_step_kernels)
+import test_gpu_sample_noise as SN   # noqa: E402
+run("keyed noise", SN.test_randn_keyed_matches_numpy_philox, 13, 1, 0)
+run("keyed steps", SN.test_keyed_step_equals_batch_step_fed_keyed_noise_and_table_form, 7, 0.6)
+run("keyed bad args", SN.test_bad_keyed_arguments_are_rejected_and_launch_nothing)
 if what != "ops-no-res1":
     run("gemm", T.test_gemm, 128 * 170 + 5, 768, 1024, 0, 0, True, True, 0)   # persistent tiles wrap, residual epilogue
 if what == "all":
