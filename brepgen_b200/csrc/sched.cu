@@ -191,6 +191,72 @@ __global__ void __launch_bounds__(256) ddpm_step_keyed_kernel(const DdpmKeyedP p
   }
 }
 
+// DDIM step (diffusers 0.27 DDIMScheduler.step, epsilon prediction), diffusers' order of operations in fp32:
+//   x0 = (x - sb*e) / sa, clamped to +-clip;  e_dir = e, or (x - sa*x0) / sb with use_clipped_eps;
+//   out = sa_prev*x0 + c_dir*e_dir [+ sigma*z].
+// One kernel serves every form.  Noise: explicit `noise`, else per-sample keys (keyed_normal4, domain 0, timestep t: the
+// normals the keyed DDPM step draws at the same t), else the batch stream (seed, offset + element_group) of
+// ddpm_step_kernel.  Table form (coef != NULL): coefficients (sb, sa, sa_prev, c_dir, sigma) from coef[*step], t from
+// *t_cur and the batch-stream offset offset + k * offset_stride.  Without keys the whole tensor is one "sample"
+// (per_sample = n), so the group index is the batch stream's element group.
+struct DdimP {
+  const float *eps_c, *eps_u, *x, *noise;
+  float* out;
+  long long n, per_sample;
+  float w, sb, sa, sa_prev, c_dir, sigma, clip;
+  int use_clipped_eps;
+  const unsigned long long* keys;
+  long long t;
+  unsigned long long seed, offset, offset_stride;
+  const float* coef;
+  const int* step;
+  const long long* t_cur;
+};
+__global__ void __launch_bounds__(256) ddim_step_kernel(const DdimP p) {
+  float sb = p.sb, sa = p.sa, sa_prev = p.sa_prev, c_dir = p.c_dir, sigma = p.sigma;
+  long long t = p.t;
+  unsigned long long offset = p.offset;
+  if (p.coef) {
+    const int k = *p.step;
+    const float* cf = p.coef + 5 * (long long)k;
+    sb = cf[0]; sa = cf[1]; sa_prev = cf[2]; c_dir = cf[3]; sigma = cf[4];
+    if (p.t_cur) t = *p.t_cur;
+    offset += (unsigned long long)k * p.offset_stride;
+  }
+  const long long gps = (p.per_sample + 3) / 4, ng = (p.n / p.per_sample) * gps;
+  for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += (long long)gridDim.x * blockDim.x) {
+    const long long b = g / gps, q = g - b * gps;
+    float z[4] = {0.f, 0.f, 0.f, 0.f};
+    if (sigma != 0.f && p.noise == nullptr) {
+      if (p.keys) {
+        keyed_normal4(p.keys[b], (unsigned long long)q, (uint32_t)t, 0u, z);
+      } else {
+        uint32_t r[4];
+        const unsigned long long ctr = offset + (unsigned long long)q;
+        philox4x32_10((uint32_t)ctr, (uint32_t)(ctr >> 32), 0u, 0u, (uint32_t)p.seed, (uint32_t)(p.seed >> 32), r);
+        box_muller(r[0], r[1], z[0], z[1]);
+        box_muller(r[2], r[3], z[2], z[3]);
+      }
+    }
+    const long long base = b * p.per_sample;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const long long js = q * 4 + j;
+      if (js >= p.per_sample) break;
+      const long long i = base + js;
+      float e = p.eps_c[i];
+      if (p.eps_u) e = e * (1.f + p.w) - p.eps_u[i] * p.w;
+      const float xv = p.x[i];
+      float x0 = (xv - sb * e) / sa;
+      if (p.clip > 0.f) x0 = fminf(fmaxf(x0, -p.clip), p.clip);
+      if (p.use_clipped_eps) e = (xv - sa * x0) / sb;
+      float o = sa_prev * x0 + c_dir * e;
+      if (sigma != 0.f) o += sigma * (p.noise ? p.noise[i] : z[j]);
+      p.out[i] = o;
+    }
+  }
+}
+
 // one thread: k = ++(*step);  *t_cur = ts[k]   (the denoiser reads its timestep from t_cur, the step kernel reads k)
 __global__ void step_advance_kernel(const long long* __restrict__ ts, int n, int* __restrict__ step, long long* __restrict__ t_cur) {
   int k = *step + 1;
@@ -303,6 +369,44 @@ int bg_ddpm_step_tab_keyed(const float* eps_cond, const float* eps_uncond, float
   ddpm_step_keyed_kernel<<<grid_for((n / per_sample) * ((per_sample + 3) / 4)), 256, 0,
                            reinterpret_cast<cudaStream_t>(stream)>>>(p);
   return check_launch("ddpm_step_keyed_kernel launch");
+}
+
+static int launch_ddim(DdimP& p, const uint64_t* sample_keys, int64_t per_sample, void* stream) {
+  p.keys = reinterpret_cast<const unsigned long long*>(sample_keys);
+  p.per_sample = sample_keys ? per_sample : p.n;
+  ddim_step_kernel<<<grid_for((p.n / p.per_sample) * ((p.per_sample + 3) / 4)), 256, 0,
+                     reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch("ddim_step_kernel launch");
+}
+
+int bg_ddim_step(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
+                 const float* noise, uint64_t seed, uint64_t offset, const uint64_t* sample_keys, int64_t per_sample,
+                 int64_t t, int64_t n, float sqrt_one_minus_abar, float sqrt_abar, float sqrt_abar_prev, float c_dir,
+                 float sigma, float clip, int32_t use_clipped_eps, void* stream) {
+  BG_REQUIRE(eps_cond && x && out && n > 0, "ddim_step: bad arguments");
+  BG_REQUIRE(!sample_keys || (per_sample > 0 && n % per_sample == 0),
+             "ddim_step: n must be a positive multiple of per_sample");
+  BG_REQUIRE(t >= 0 && t <= 0xFFFFFFFFll, "ddim_step: t must be a 32-bit unsigned value");
+  BG_REQUIRE(sqrt_abar > 0.f, "ddim_step: sqrt_abar must be positive");
+  DdimP p = {};
+  p.eps_c = eps_cond; p.eps_u = eps_uncond; p.x = x; p.noise = noise; p.out = out; p.n = n;
+  p.w = cfg_w; p.sb = sqrt_one_minus_abar; p.sa = sqrt_abar; p.sa_prev = sqrt_abar_prev; p.c_dir = c_dir; p.sigma = sigma;
+  p.clip = clip; p.use_clipped_eps = use_clipped_eps != 0; p.t = t; p.seed = seed; p.offset = offset;
+  return launch_ddim(p, sample_keys, per_sample, stream);
+}
+
+int bg_ddim_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out, uint64_t seed,
+                     uint64_t offset0, uint64_t offset_stride, const uint64_t* sample_keys, int64_t per_sample,
+                     const int64_t* t_cur, int64_t n, const float* coef_table, const int32_t* step, float clip,
+                     int32_t use_clipped_eps, void* stream) {
+  BG_REQUIRE(eps_cond && x && out && n > 0 && coef_table && step, "ddim_step_tab: bad arguments");
+  BG_REQUIRE(!sample_keys || (t_cur && per_sample > 0 && n % per_sample == 0),
+             "ddim_step_tab: keyed noise needs t_cur and n a positive multiple of per_sample");
+  DdimP p = {};
+  p.eps_c = eps_cond; p.eps_u = eps_uncond; p.x = x; p.out = out; p.n = n; p.w = cfg_w; p.clip = clip;
+  p.use_clipped_eps = use_clipped_eps != 0; p.seed = seed; p.offset = offset0; p.offset_stride = offset_stride;
+  p.coef = coef_table; p.step = step; p.t_cur = reinterpret_cast<const long long*>(t_cur);
+  return launch_ddim(p, sample_keys, per_sample, stream);
 }
 
 int bg_step_advance(const int64_t* timesteps, int n_steps, int32_t* step, int64_t* t_cur, void* stream) {

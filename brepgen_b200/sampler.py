@@ -5,8 +5,9 @@ Same stage order, tensor shapes, late face-count increase (sample.py:140-142), c
 reshapes (sample.py:284-294).  Differences, all result-preserving:
   * no D2H/H2D round trips: dedup runs as device kernels (csrc/dedup.cu), timesteps are device-resident views;
   * CFG combine is fused into the DDPM update kernel (PNDM steps combine with one bg_axpby);
-  * two schedules: "reference" = the shipped PNDM(200)[:158] + DDPM(1000)[-250:] hybrid, and "ddpm" = N DDPM steps for
-    every stage, which is BASELINE.json's benchmark definition (N = 1000).
+  * three schedules: "reference" = the shipped PNDM(200)[:158] + DDPM(1000)[-250:] hybrid, "ddpm" = N DDPM steps for
+    every stage, which is BASELINE.json's benchmark definition (N = 1000), and "ddim" = N DDIM steps for every stage
+    (few-step sampling of the same DDPM-trained denoisers).
 Everything past sample.py:299 (OpenCASCADE post-processing) is out of scope (SURVEY.md section 2).
 
 Batch sharding across GPUs: samples are independent through every stage, so each rank runs its own shard and there is
@@ -20,7 +21,7 @@ from typing import Dict, List, Optional, Sequence
 import torch
 
 from . import _ffi
-from .schedulers import DDPMScheduler, PNDMScheduler, sample_keys, sample_seed
+from .schedulers import DDIMScheduler, DDPMScheduler, PNDMScheduler, sample_keys, sample_seed
 
 NOISE_MODES = ("batch", "per_sample")
 
@@ -37,8 +38,10 @@ class CascadeConfig:
     class_label: int = 0                 # TEXT2INT[...] when use_cf
     bbox_threshold: float = 0.08         # eval_config.yaml:10
     guidance_w: float = 0.6              # sample.py:49
-    schedule: str = "reference"          # "reference" | "ddpm"
+    schedule: str = "reference"          # "reference" | "ddpm" | "ddim"
     ddpm_steps: int = 1000               # per stage, schedule == "ddpm"
+    ddim_steps: int = 50                 # per stage, schedule == "ddim"
+    ddim_eta: float = 0.0                # schedule == "ddim": 0 = deterministic DDIM, 1 = DDPM-like noise
     dense_masks: bool = False            # True: skip dedup, every slot valid (the dense-FLOP benchmark mode)
     ragged_masks: bool = False           # benchmark only: synthetic masks shaped like a trained model's output (random-init
                                          # weights never produce duplicates): 1/8..1/2 of the faces valid, 3..E/3 edges each
@@ -132,6 +135,15 @@ def per_sample_seeds(cfg: CascadeConfig) -> Optional[List[int]]:
     return [sample_seed(int(cfg.seed), int(cfg.sample_base) + b) for b in range(cfg.batch_size)]
 
 
+def check_schedule(cfg: CascadeConfig) -> None:
+    """raises ValueError on out-of-range DDIM settings (ddim_steps outside [1, 1000], ddim_eta < 0)"""
+    if cfg.schedule == "ddim":
+        if not 1 <= int(cfg.ddim_steps) <= 1000:
+            raise ValueError(f"CascadeConfig.ddim_steps must be in [1, 1000], got {cfg.ddim_steps}")
+        if not float(cfg.ddim_eta) >= 0.0:
+            raise ValueError(f"CascadeConfig.ddim_eta must be >= 0, got {cfg.ddim_eta}")
+
+
 def randn_keyed(seeds: Sequence[int], stage: int, shape, device, domain: int = 1, t: int = 0) -> torch.Tensor:
     """(len(seeds), *shape[1:]) fp32 normals from the per-sample streams (bg_randn_keyed); default domain 1 = initial noise"""
     B = len(seeds)
@@ -178,6 +190,9 @@ class Cascade:
                                   beta_start=0.0001, beta_end=0.02)
         self.ddpm = DDPMScheduler(num_train_timesteps=1000, beta_schedule="linear", prediction_type="epsilon",
                                   beta_start=0.0001, beta_end=0.02, clip_sample=True, clip_sample_range=3)
+        self.ddim = DDIMScheduler(num_train_timesteps=1000, beta_schedule="linear", prediction_type="epsilon",
+                                  beta_start=0.0001, beta_end=0.02, clip_sample=True, clip_sample_range=3,
+                                  set_alpha_to_one=True)
 
     # ------------------------------------------------------------------ one DDPM loop as a replayed CUDA graph
     def _use_graph(self, cfg: CascadeConfig, n_steps: int, tokens: int) -> bool:
@@ -188,28 +203,31 @@ class Cascade:
         # a forward is ~105 launches from Python (~1 ms of host time); below ~100 k tokens the GPU finishes sooner than that
         return n_steps >= 32 and tokens <= 100_000
 
-    def _loop_graph(self, cfg: CascadeConfig, timesteps, x, fwd):
-        """timesteps: 1-D int64 CPU tensor; x: (B, ...) fp32 on the device; fwd(x_in, t_dev) -> eps of a (possibly CFG-doubled)
-        batch.  The loop body of sample.py:145-153 -- [step counter / timestep advance] -> forward -> fused scheduler step
-        (CFG combine, x0, clip, posterior mean, Philox noise) -- is captured ONCE and replayed len(timesteps) times: no
-        per-step host work.  Nothing step-specific is a kernel argument: the timestep comes from a device scalar, the
-        coefficients from a device table indexed by a device counter (bg_step_advance / bg_ddpm_step_tab)."""
+    def _loop_graph(self, cfg: CascadeConfig, sched, timesteps, x, fwd):
+        """sched: self.ddpm or self.ddim; timesteps: 1-D int64 CPU tensor; x: (B, ...) fp32 on the device; fwd(x_in, t_dev)
+        -> eps of a (possibly CFG-doubled) batch.  The loop body of sample.py:145-153 -- [step counter / timestep advance] ->
+        forward -> fused scheduler step (CFG combine, x0, clip, DDPM posterior mean or DDIM update, Philox noise) -- is
+        captured ONCE and replayed len(timesteps) times: no per-step host work.  Nothing step-specific is a kernel argument:
+        the timestep comes from a device scalar, the coefficients from a device table indexed by a device counter
+        (bg_step_advance / bg_ddpm_step_tab / bg_ddim_step_tab)."""
         dev = self.device
         lib = _ffi.lib()
         T = len(timesteps)
         B = x.shape[0]
         xb = x.detach().float().contiguous().clone()
         n = xb.numel()
-        coef = self.ddpm.coefficient_table(timesteps).to(dev)
+        ddim = isinstance(sched, DDIMScheduler)
+        coef = (sched.coefficient_table(timesteps, cfg.ddim_eta) if ddim else sched.coefficient_table(timesteps)).to(dev)
         ts = timesteps.to(device=dev, dtype=torch.int64).contiguous()
         step = torch.full((1,), -1, dtype=torch.int32, device=dev)
         t_cur = torch.zeros(1, dtype=torch.int64, device=dev)
-        keyed = self.ddpm.per_sample_noise
+        keyed = sched.per_sample_noise
+        seed, off0, stride, keys = 0, 0, 0, None
         if keyed:     # per-sample streams counted by the device timestep t_cur: no offset to carry between graphs
-            keys = self.ddpm.sample_key_tensor(B, dev)
+            keys = sched.sample_key_tensor(B, dev)
         else:
-            seed, off0, stride = self.ddpm.philox_stream(n)
-        clip = float(self.ddpm.config.clip_sample_range) if self.ddpm.config.clip_sample else 0.0
+            seed, off0, stride = sched.philox_stream(n)
+        clip = float(sched.config.clip_sample_range) if sched.config.clip_sample else 0.0
 
         def body():
             st = _ffi.current_stream()
@@ -217,6 +235,11 @@ class Cascade:
             pred = fwd(torch.cat([xb, xb], 0) if cfg.use_cf else xb, t_cur)
             pc = pred[:B] if cfg.use_cf else pred
             pu = pred[B:] if cfg.use_cf else None
+            if ddim:
+                _ffi.check(lib.bg_ddim_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(),
+                                                xb.data_ptr(), seed, off0, stride, _ffi.ptr(keys), n // B, t_cur.data_ptr(),
+                                                n, coef.data_ptr(), step.data_ptr(), clip, 0, st), "bg_ddim_step_tab")
+                return
             if keyed:
                 _ffi.check(lib.bg_ddpm_step_tab_keyed(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(),
                                                       xb.data_ptr(), keys.data_ptr(), n // B, t_cur.data_ptr(), n,
@@ -243,18 +266,18 @@ class Cascade:
         for _ in range(T):
             g.replay()
         _ffi.note_replay(per_replay, T)
-        if not keyed:
-            self.ddpm.advance_philox(n, T)
+        if not keyed and (not ddim or cfg.ddim_eta > 0):     # DDIM draws (and advances the stream) only when eta > 0
+            sched.advance_philox(n, T)
         self.last_graph_steps = getattr(self, "last_graph_steps", 0) + T
         return xb
 
     # ------------------------------------------------------------------ one denoising loop
     def _loop(self, cfg: CascadeConfig, sched, timesteps, x, fwd, label2, gen, on_step=None, noise_fn=None):
-        """fwd(x_in, t_dev) -> eps for a (possibly CFG-doubled) batch; noise_fn(k, shape) -> explicit DDPM step noise"""
+        """fwd(x_in, t_dev) -> eps for a (possibly CFG-doubled) batch; noise_fn(k, shape) -> explicit DDPM / DDIM step noise"""
         B = x.shape[0]
         k = 0
-        is_ddpm = isinstance(sched, DDPMScheduler)
-        if is_ddpm and noise_fn is None and gen is None and len(timesteps) > 0 and \
+        fused = isinstance(sched, (DDPMScheduler, DDIMScheduler))    # CFG combine and noise inside the step kernel
+        if fused and noise_fn is None and gen is None and len(timesteps) > 0 and \
                 self._use_graph(cfg, len(timesteps), x[0].numel() // x.shape[-1] * B * (2 if cfg.use_cf else 1)):
             # on_step (the late face-count increase, sample.py:140-142) changes the shape once: one graph per segment
             lo = 0
@@ -268,7 +291,7 @@ class Cascade:
                         hi += 1
                 else:
                     hi = len(ts_list)
-                x = self._loop_graph(cfg, timesteps[lo:hi], x, fwd)
+                x = self._loop_graph(cfg, sched, timesteps[lo:hi], x, fwd)
                 lo = hi
             return x
         ts_dev = timesteps.to(self.device)
@@ -280,10 +303,9 @@ class Cascade:
                 B = x.shape[0]
             if cfg.use_cf:
                 pred = fwd(torch.cat([x, x], 0), t_dev)
-                if is_ddpm:
-                    nz = noise_fn(k, x.shape).to(self.device) if (noise_fn is not None and int(t) > 0) else None
-                    x = sched.step(pred[:B], t, x, generator=gen, noise=nz, model_output_uncond=pred[B:],
-                                   guidance_w=cfg.guidance_w).prev_sample
+                if fused:
+                    x = self._fused_step(cfg, sched, k, t, x, pred[:B], gen, noise_fn, model_output_uncond=pred[B:],
+                                         guidance_w=cfg.guidance_w)
                 else:
                     eps = torch.empty_like(x)
                     w = cfg.guidance_w
@@ -292,22 +314,34 @@ class Cascade:
                     x = sched.step(eps, t, x).prev_sample
             else:
                 pred = fwd(x, t_dev)
-                if is_ddpm:
-                    nz = noise_fn(k, x.shape).to(self.device) if (noise_fn is not None and int(t) > 0) else None
-                    x = sched.step(pred, t, x, generator=gen, noise=nz).prev_sample
+                if fused:
+                    x = self._fused_step(cfg, sched, k, t, x, pred, gen, noise_fn)
                 else:
                     x = sched.step(pred, t, x).prev_sample
             k += 1
         return x
 
+    def _fused_step(self, cfg, sched, k, t, x, pred, gen, noise_fn, **cf):
+        """one DDPM or DDIM step; explicit noise from noise_fn on the steps where diffusers draws it: DDPM at t > 0, DDIM
+        on every step when eta > 0"""
+        if isinstance(sched, DDIMScheduler):
+            nz = noise_fn(k, x.shape).to(self.device) if (noise_fn is not None and cfg.ddim_eta > 0) else None
+            return sched.step(pred, t, x, eta=cfg.ddim_eta, generator=gen, variance_noise=nz, **cf).prev_sample
+        nz = noise_fn(k, x.shape).to(self.device) if (noise_fn is not None and int(t) > 0) else None
+        return sched.step(pred, t, x, generator=gen, noise=nz, **cf).prev_sample
+
     _STAGE_ID = {"surfPos": 0, "surfZ": 1, "edgePos": 2, "edgeZV": 3}
 
     def _stage(self, cfg, x, fwd, label2, gen, hybrid_ddpm_tail: bool, on_step=None, noise_fn=None, name="surfPos"):
         seeds = getattr(self, "_sample_seeds", None)
+        noisy = self.ddim if cfg.schedule == "ddim" else self.ddpm
         if seeds is not None:
-            self.ddpm.set_sample_keys(sample_seeds=seeds, stage=self._STAGE_ID[name])
+            noisy.set_sample_keys(sample_seeds=seeds, stage=self._STAGE_ID[name])
         else:
-            self.ddpm.set_noise_seed(*getattr(self, "_noise_key", (int(cfg.seed), 0)), self._STAGE_ID[name])
+            noisy.set_noise_seed(*getattr(self, "_noise_key", (int(cfg.seed), 0)), self._STAGE_ID[name])
+        if cfg.schedule == "ddim":
+            self.ddim.set_timesteps(cfg.ddim_steps)
+            return self._loop(cfg, self.ddim, self.ddim.timesteps, x, fwd, label2, gen, on_step, noise_fn)
         if cfg.schedule == "ddpm":
             self.ddpm.set_timesteps(cfg.ddpm_steps)
             return self._loop(cfg, self.ddpm, self.ddpm.timesteps, x, fwd, label2, gen, on_step, noise_fn)
@@ -325,10 +359,12 @@ class Cascade:
     # ------------------------------------------------------------------ the cascade
     @torch.no_grad()
     def run(self, cfg: CascadeConfig, init_noise: Optional[Dict[str, torch.Tensor]] = None, step_noise=None):
-        """step_noise(stage_name, k, shape) -> tensor: explicit DDPM step noise (parity runs); default = in-kernel Philox
+        """step_noise(stage_name, k, shape) -> tensor: explicit DDPM / DDIM step noise of step k (parity runs; DDPM draws it
+        at t > 0, DDIM on every step when ddim_eta > 0); default = in-kernel Philox
         keyed by (cfg.seed, rank, stage): reproducible from cfg.seed, independent across ranks and stages.
         cfg.noise == "per_sample": initial and step noise come from each sample's own streams (bg_randn_keyed and the keyed
         step kernels), so sample b's outputs depend on its seed alone; init_noise / step_noise still take precedence."""
+        check_schedule(cfg)
         seeds = per_sample_seeds(cfg)
         self._sample_seeds = seeds
         dev = self.device

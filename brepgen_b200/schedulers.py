@@ -1,4 +1,5 @@
-"""Drop-in DDPMScheduler / PNDMScheduler with the diffusers 0.27 interface used by the reference.
+"""Drop-in DDPMScheduler / PNDMScheduler with the diffusers 0.27 interface used by the reference, and DDIMScheduler
+(diffusers' few-step sampler for the same epsilon-prediction models; not used by the reference).
 
 Call sites mirrored (all in the reference): constructors sample.py:101-117 and trainer.py:285-292;
 `set_timesteps(n)` + `.timesteps[...]` slicing sample.py:128-129,144-145; `.step(pred, t, x).prev_sample`
@@ -6,7 +7,7 @@ sample.py:137,153,202,222,236,282; `.add_noise(x, noise, t)` trainer.py:348; `.c
 
 Host side (this file): the beta / alphas_cumprod tables and the per-step scalar coefficients, computed with the same
 fp32 torch-CPU operations diffusers uses (SURVEY.md Appendix A.3/A.4).  Device side: ONE fused kernel per step
-(bg_ddpm_step / bg_pndm_step in csrc/sched.cu) instead of ~15 scalar-broadcast launches.  No CPU tensor path:
+(bg_ddpm_step / bg_ddim_step / bg_pndm_step in csrc/sched.cu) instead of ~15 scalar-broadcast launches.  No CPU tensor path:
 `step` on a CPU sample raises.
 """
 from __future__ import annotations
@@ -80,26 +81,43 @@ def _require_cuda(x: torch.Tensor, what: str):
         raise RuntimeError(f"brepgen_b200 schedulers have no CPU path: {what} must be a CUDA tensor")
 
 
-class DDPMScheduler:
-    def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.0001, beta_end: float = 0.02,
-                 beta_schedule: str = "linear", prediction_type: str = "epsilon", clip_sample: bool = True,
-                 clip_sample_range: float = 1.0, variance_type: str = "fixed_small", **unused):
-        if prediction_type != "epsilon" or variance_type != "fixed_small":
-            raise NotImplementedError("only prediction_type='epsilon', variance_type='fixed_small' (sample.py:109-117)")
-        self.config = SimpleNamespace(num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
-                                      beta_schedule=beta_schedule, prediction_type=prediction_type,
-                                      clip_sample=clip_sample, clip_sample_range=clip_sample_range,
-                                      variance_type=variance_type)
-        self.betas = _betas(num_train_timesteps, beta_start, beta_end, beta_schedule)
-        self.alphas = 1.0 - self.betas
-        self.alphas_cumprod = torch.cumprod(self.alphas, dim=0)
-        self.one = torch.tensor(1.0)
-        self.init_noise_sigma = 1.0
+def _step_tensors(what, model_output, sample, model_output_uncond, noise, out):
+    """Checks the tensors of a fused step; returns (x, eps, eps_uncond, destination) as contiguous fp32."""
+    # the C ABI takes raw pointers and one element count: every tensor must cover exactly sample.numel() elements
+    for name, ten in (("model_output", model_output), ("model_output_uncond", model_output_uncond), ("noise", noise),
+                      ("out", out)):
+        if ten is not None and tuple(ten.shape) != tuple(sample.shape):
+            raise RuntimeError(f"{what}: {name} has shape {tuple(ten.shape)}, sample has {tuple(sample.shape)}")
+    if out is not None and (out.dtype != torch.float32 or not out.is_contiguous() or out.device != sample.device):
+        raise RuntimeError(f"{what}: `out` must be a contiguous fp32 tensor on the sample's device")
+    _require_cuda(sample, "sample")
+    _require_cuda(model_output, "model_output")
+    x = sample if (sample.dtype == torch.float32 and sample.is_contiguous()) else sample.float().contiguous()
+    eps = model_output.float().contiguous()
+    eps_u = None if model_output_uncond is None else model_output_uncond.float().contiguous()
+    return x, eps, eps_u, (torch.empty_like(x) if out is None else out)
+
+
+def _generator_noise(x: torch.Tensor, generator) -> torch.Tensor:
+    """N(0, 1) of x's shape drawn as diffusers' randn_tensor draws it from `generator` (one, or a list with one per batch
+    element)"""
+    if isinstance(generator, (list, tuple)):
+        # diffusers' randn_tensor with one generator per batch element (the reference's utils.py:62-97)
+        return randn_generators(x.shape, generator, x.device)
+    # diffusers' randn_tensor: a CPU generator samples on the CPU and the result is moved to the device
+    gdev = generator.device if hasattr(generator, "device") else torch.device("cpu")
+    return torch.randn(x.shape, generator=generator, device=x.device if gdev.type == "cuda" else "cpu", dtype=torch.float32)
+
+
+class _NoiseStreams:
+    """The in-kernel noise sources shared by the fused DDPM and DDIM steps: one batch-wide Philox stream
+    (set_noise_seed) or per-sample streams (set_sample_keys)."""
+
+    def _init_noise_streams(self):
         self._philox_seed = None       # None: derived from torch.initial_seed() at first use (follows torch.manual_seed)
         self._philox_offset = 0
         self._sample_seeds = None      # per-sample noise mode: None (batch-wide stream) or (seed, first, stage, seeds)
         self._key_cache = {}
-        self.set_timesteps(num_train_timesteps)
 
     def set_noise_seed(self, seed: int, *stream: int):
         """Key of the in-kernel Philox stream that `step` draws its noise from when neither `noise` nor `generator` is
@@ -126,16 +144,45 @@ class DDPMScheduler:
     def sample_key_tensor(self, batch: int, device) -> torch.Tensor:
         """device int64 [batch] holding the uint64 keys of the per-sample mode set by set_sample_keys"""
         if self._sample_seeds is None:
-            raise RuntimeError("DDPMScheduler: per-sample noise mode is not set (call set_sample_keys)")
+            raise RuntimeError(f"{type(self).__name__}: per-sample noise mode is not set (call set_sample_keys)")
         seed, first, stage, seeds = self._sample_seeds
         if seeds is None:
             seeds = [sample_seed(seed, first + i) for i in range(batch)]
         elif len(seeds) != batch:
-            raise ValueError(f"DDPMScheduler: {len(seeds)} sample seeds for a batch of {batch}")
+            raise ValueError(f"{type(self).__name__}: {len(seeds)} sample seeds for a batch of {batch}")
         key = (batch, str(device))
         if key not in self._key_cache:
             self._key_cache[key] = torch.from_numpy(sample_keys(seeds, stage).view(np.int64)).to(device)
         return self._key_cache[key]
+
+    def philox_stream(self, n: int):
+        """(seed, offset0, stride) of the in-kernel noise stream for a loop of steps over n elements; advances the
+        scheduler's offset past `steps` later via advance_philox."""
+        if self._philox_seed is None:
+            self._philox_seed = mix_seed(torch.initial_seed())
+        return self._philox_seed, self._philox_offset, (n + 3) // 4
+
+    def advance_philox(self, n: int, steps: int):
+        self._philox_offset += steps * ((n + 3) // 4)
+
+
+class DDPMScheduler(_NoiseStreams):
+    def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.0001, beta_end: float = 0.02,
+                 beta_schedule: str = "linear", prediction_type: str = "epsilon", clip_sample: bool = True,
+                 clip_sample_range: float = 1.0, variance_type: str = "fixed_small", **unused):
+        if prediction_type != "epsilon" or variance_type != "fixed_small":
+            raise NotImplementedError("only prediction_type='epsilon', variance_type='fixed_small' (sample.py:109-117)")
+        self.config = SimpleNamespace(num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
+                                      beta_schedule=beta_schedule, prediction_type=prediction_type,
+                                      clip_sample=clip_sample, clip_sample_range=clip_sample_range,
+                                      variance_type=variance_type)
+        self.betas = _betas(num_train_timesteps, beta_start, beta_end, beta_schedule)
+        self.alphas = 1.0 - self.betas
+        self.alphas_cumprod = torch.cumprod(self.alphas, dim=0)
+        self.one = torch.tensor(1.0)
+        self.init_noise_sigma = 1.0
+        self._init_noise_streams()
+        self.set_timesteps(num_train_timesteps)
 
     def set_timesteps(self, num_inference_steps: int, device=None):
         n_train = self.config.num_train_timesteps
@@ -170,16 +217,6 @@ class DDPMScheduler:
         rows = [self.step_coefficients(_as_int(t)) for t in timesteps]
         return torch.tensor(rows, dtype=torch.float32).reshape(-1, 5)
 
-    def philox_stream(self, n: int):
-        """(seed, offset0, stride) of the in-kernel noise stream for a loop of steps over n elements; advances the
-        scheduler's offset past `steps` later via advance_philox."""
-        if self._philox_seed is None:
-            self._philox_seed = mix_seed(torch.initial_seed())
-        return self._philox_seed, self._philox_offset, (n + 3) // 4
-
-    def advance_philox(self, n: int, steps: int):
-        self._philox_offset += steps * ((n + 3) // 4)
-
     def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, generator=None, return_dict: bool = True,
              noise: Optional[torch.Tensor] = None, model_output_uncond: Optional[torch.Tensor] = None,
              guidance_w: float = 0.0, out: Optional[torch.Tensor] = None):
@@ -189,33 +226,14 @@ class DDPMScheduler:
         diffusers, a list with one per batch element (sample i's noise from generator[i]; CPU generators sample on the
         host).  Without `noise` or `generator` the noise comes from the in-kernel stream: batch-wide (set_noise_seed) or
         per sample (set_sample_keys)."""
-        # the C ABI takes raw pointers and one element count: every tensor must cover exactly sample.numel() elements
-        for name, ten in (("model_output", model_output), ("model_output_uncond", model_output_uncond), ("noise", noise),
-                          ("out", out)):
-            if ten is not None and tuple(ten.shape) != tuple(sample.shape):
-                raise RuntimeError(f"DDPMScheduler.step: {name} has shape {tuple(ten.shape)}, sample has {tuple(sample.shape)}")
-        if out is not None and (out.dtype != torch.float32 or not out.is_contiguous() or out.device != sample.device):
-            raise RuntimeError("DDPMScheduler.step: `out` must be a contiguous fp32 tensor on the sample's device")
-        _require_cuda(sample, "sample")
-        _require_cuda(model_output, "model_output")
+        x, eps, eps_u, dst = _step_tensors("DDPMScheduler.step", model_output, sample, model_output_uncond, noise, out)
         t = _as_int(timestep)
         sb, sa, c_x0, c_x, sigma = self.step_coefficients(t)
-        x = sample if (sample.dtype == torch.float32 and sample.is_contiguous()) else sample.float().contiguous()
-        eps = model_output.float().contiguous()
-        eps_u = None if model_output_uncond is None else model_output_uncond.float().contiguous()
         if noise is None and generator is not None and sigma != 0.0:
-            if isinstance(generator, (list, tuple)):
-                # diffusers' randn_tensor with one generator per batch element (the reference's utils.py:62-97)
-                noise = randn_generators(x.shape, generator, x.device)
-            else:
-                # diffusers' randn_tensor: a CPU generator samples on the CPU and the result is moved to the device
-                gdev = generator.device if hasattr(generator, "device") else torch.device("cpu")
-                noise = torch.randn(x.shape, generator=generator, device=x.device if gdev.type == "cuda" else "cpu",
-                                    dtype=torch.float32)
+            noise = _generator_noise(x, generator)
         if noise is not None:
             noise = noise.to(device=x.device, dtype=torch.float32).contiguous()
         n = x.numel()
-        dst = torch.empty_like(x) if out is None else out
         clip = float(self.config.clip_sample_range) if self.config.clip_sample else 0.0
         if self._sample_seeds is not None:
             keys = self.sample_key_tensor(x.shape[0], x.device)
@@ -246,6 +264,111 @@ class DDPMScheduler:
         while sa.dim() < original_samples.dim():
             sa, sb = sa.unsqueeze(-1), sb.unsqueeze(-1)
         return sa * original_samples + sb * noise
+
+    def __len__(self):
+        return self.config.num_train_timesteps
+
+
+class DDIMScheduler(_NoiseStreams):
+    """diffusers 0.27 DDIMScheduler for epsilon-prediction models: few-step deterministic (eta = 0) or stochastic sampling
+    of a model trained as a DDPM.  One fused kernel per step (bg_ddim_step); the per-step scalars are computed here in fp32
+    torch as diffusers computes them."""
+
+    def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.0001, beta_end: float = 0.02,
+                 beta_schedule: str = "linear", trained_betas=None, clip_sample: bool = True, set_alpha_to_one: bool = True,
+                 steps_offset: int = 0, prediction_type: str = "epsilon", thresholding: bool = False,
+                 dynamic_thresholding_ratio: float = 0.995, clip_sample_range: float = 1.0, sample_max_value: float = 1.0,
+                 timestep_spacing: str = "leading", rescale_betas_zero_snr: bool = False, **unused):
+        if prediction_type != "epsilon" or thresholding or rescale_betas_zero_snr or timestep_spacing != "leading" or \
+                trained_betas is not None:
+            raise NotImplementedError("only prediction_type='epsilon', timestep_spacing='leading', no thresholding, no "
+                                      "zero-SNR rescaling and no trained_betas")
+        self.config = SimpleNamespace(num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
+                                      beta_schedule=beta_schedule, trained_betas=trained_betas, clip_sample=clip_sample,
+                                      set_alpha_to_one=set_alpha_to_one, steps_offset=steps_offset,
+                                      prediction_type=prediction_type, thresholding=thresholding,
+                                      dynamic_thresholding_ratio=dynamic_thresholding_ratio,
+                                      clip_sample_range=clip_sample_range, sample_max_value=sample_max_value,
+                                      timestep_spacing=timestep_spacing, rescale_betas_zero_snr=rescale_betas_zero_snr)
+        self.betas = _betas(num_train_timesteps, beta_start, beta_end, beta_schedule)
+        self.alphas = 1.0 - self.betas
+        self.alphas_cumprod = torch.cumprod(self.alphas, dim=0)
+        self.final_alpha_cumprod = torch.tensor(1.0) if set_alpha_to_one else self.alphas_cumprod[0]
+        self.init_noise_sigma = 1.0
+        self.num_inference_steps = None
+        self.timesteps = torch.from_numpy(np.arange(0, num_train_timesteps)[::-1].copy().astype(np.int64))
+        self._init_noise_streams()
+
+    def set_timesteps(self, num_inference_steps: int, device=None):
+        n_train = self.config.num_train_timesteps
+        if num_inference_steps > n_train:
+            raise ValueError("num_inference_steps cannot exceed num_train_timesteps")
+        self.num_inference_steps = num_inference_steps
+        ratio = n_train // num_inference_steps                      # timestep_spacing = "leading"
+        ts = (np.arange(0, num_inference_steps) * ratio).round()[::-1].copy().astype(np.int64)
+        self.timesteps = torch.from_numpy(ts + self.config.steps_offset)
+
+    def scale_model_input(self, sample, timestep=None):
+        return sample
+
+    def step_coefficients(self, t: int, eta: float = 0.0):
+        """(sqrt(1-abar_t), sqrt(abar_t), sqrt(abar_prev), c_dir, sigma) as Python floats (fp32 arithmetic like diffusers)"""
+        if self.num_inference_steps is None:
+            raise ValueError("Number of inference steps is 'None', you need to run 'set_timesteps' after creating the "
+                             "scheduler")
+        prev_t = t - self.config.num_train_timesteps // self.num_inference_steps
+        a_t = self.alphas_cumprod[t]
+        a_prev = self.alphas_cumprod[prev_t] if prev_t >= 0 else self.final_alpha_cumprod
+        b_t = 1 - a_t
+        variance = ((1 - a_prev) / b_t) * (1 - a_t / a_prev)
+        std_dev_t = eta * variance ** 0.5
+        c_dir = (1 - a_prev - std_dev_t ** 2) ** 0.5
+        return float(b_t ** 0.5), float(a_t ** 0.5), float(a_prev ** 0.5), float(c_dir), float(std_dev_t)
+
+    def coefficient_table(self, timesteps, eta: float = 0.0) -> torch.Tensor:
+        """[len(timesteps), 5] fp32 (CPU): step_coefficients(t, eta) for every t of a denoising loop -- the device table
+        that bg_ddim_step_tab indexes with its step counter when the loop is captured in a CUDA graph."""
+        rows = [self.step_coefficients(_as_int(t), eta) for t in timesteps]
+        return torch.tensor(rows, dtype=torch.float32).reshape(-1, 5)
+
+    def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, eta: float = 0.0,
+             use_clipped_model_output: bool = False, generator=None, variance_noise: Optional[torch.Tensor] = None,
+             return_dict: bool = True, model_output_uncond: Optional[torch.Tensor] = None, guidance_w: float = 0.0,
+             out: Optional[torch.Tensor] = None):
+        """x_{t-1} of diffusers' DDIM step.  When eta > 0 the noise comes from `variance_noise`, else `generator` (one, or
+        a list with one per batch element), else the in-kernel stream (per sample after set_sample_keys, else batch-wide),
+        and is drawn on every step, the last one included, as diffusers draws it.  Extras over diffusers, as in
+        DDPMScheduler.step: `model_output_uncond` + `guidance_w` fuse the classifier-free combine, `out` is the
+        destination (may be `sample`).  pred_original_sample is not returned (None)."""
+        t = _as_int(timestep)
+        sb, sa, sa_prev, c_dir, sigma = self.step_coefficients(t, eta)
+        if eta > 0 and variance_noise is not None and generator is not None:
+            raise ValueError("Cannot pass both generator and variance_noise. Please make sure that either "
+                             "`generator` or `variance_noise` stays `None`.")
+        x, eps, eps_u, dst = _step_tensors("DDIMScheduler.step", model_output, sample, model_output_uncond,
+                                           variance_noise, out)
+        noise, seed, offset, keys = None, 0, 0, None
+        n = x.numel()
+        if eta > 0:
+            noise = variance_noise if variance_noise is not None else \
+                (_generator_noise(x, generator) if generator is not None else None)
+            if noise is not None:
+                noise = noise.to(device=x.device, dtype=torch.float32).contiguous()
+            elif self._sample_seeds is not None:
+                keys = self.sample_key_tensor(x.shape[0], x.device)
+            else:
+                seed, offset, _ = self.philox_stream(n)
+                self.advance_philox(n, 1)
+        with torch.cuda.device(x.device):
+            _ffi.check(_ffi.lib().bg_ddim_step(eps.data_ptr(), _ffi.ptr(eps_u), float(guidance_w), x.data_ptr(),
+                                              dst.data_ptr(), _ffi.ptr(noise), seed, offset, _ffi.ptr(keys),
+                                              n // x.shape[0], t, n, sb, sa, sa_prev, c_dir, sigma,
+                                              float(self.config.clip_sample_range) if self.config.clip_sample else 0.0,
+                                              int(bool(use_clipped_model_output)), _ffi.current_stream()), "bg_ddim_step")
+        return SchedulerOutput(dst) if return_dict else (dst,)
+
+    def add_noise(self, original_samples, noise, timesteps):
+        return DDPMScheduler.add_noise(self, original_samples, noise, timesteps)
 
     def __len__(self):
         return self.config.num_train_timesteps

@@ -173,6 +173,28 @@ int bg_ddpm_step_keyed(const float* eps_cond, const float* eps_uncond, float cfg
 int bg_ddpm_step_tab_keyed(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
                            const uint64_t* sample_keys, int64_t per_sample, const int64_t* t_cur, int64_t n,
                            const float* coef_table, const int32_t* step, float clip, void* stream);
+/* DDIM step (diffusers DDIMScheduler.step, prediction_type "epsilon"), fp32 in diffusers' order of operations:
+ * eps   = eps_cond if eps_uncond == NULL else eps_cond*(1+w) - eps_uncond*w            (CFG, as bg_ddpm_step)
+ * x0    = clamp((x - sqrt_one_minus_abar*eps) / sqrt_abar, -clip, clip)  (clip <= 0: no clamp)
+ * e_dir = eps, or (x - sqrt_abar*x0) / sqrt_one_minus_abar if use_clipped_eps (use_clipped_model_output)
+ * out   = sqrt_abar_prev*x0 + c_dir*e_dir + sigma*noise;   sigma = eta*sqrt((1-abar_prev)/(1-abar_t)*(1-abar_t/abar_prev)),
+ *         c_dir = sqrt(1 - abar_prev - sigma^2), computed by the host scheduler.
+ * noise (only read when sigma != 0): the explicit tensor if not NULL; else, when sample_keys != NULL, the per-sample
+ * streams of bg_ddpm_step_keyed (domain 0, timestep t; the same normals the keyed DDPM step draws at t); else the batch
+ * Philox stream (seed, offset) of bg_ddpm_step.  Keyed: per_sample <= 0 or n not a multiple of per_sample is
+ * BG_STATUS_BAD_ARG, as are NULL pointers, sqrt_abar <= 0 and t outside 32 bits; nothing is launched then. */
+int bg_ddim_step(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
+                 const float* noise, uint64_t seed, uint64_t offset, const uint64_t* sample_keys, int64_t per_sample,
+                 int64_t t, int64_t n, float sqrt_one_minus_abar, float sqrt_abar, float sqrt_abar_prev, float c_dir,
+                 float sigma, float clip, int32_t use_clipped_eps, void* stream);
+/* table-driven form for graph capture: coef_table[k][5] = (sqrt(1-abar_t), sqrt(abar_t), sqrt(abar_prev), c_dir, sigma)
+ * of step k = *step (bg_step_advance), batch-stream counter offset0 + k * offset_stride, or, when sample_keys != NULL, the
+ * per-sample streams at the timestep *t_cur (t_cur may be NULL only without keys).  Bit-identical to bg_ddim_step with the
+ * same coefficients and noise. */
+int bg_ddim_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out, uint64_t seed,
+                     uint64_t offset0, uint64_t offset_stride, const uint64_t* sample_keys, int64_t per_sample,
+                     const int64_t* t_cur, int64_t n, const float* coef_table, const int32_t* step, float clip,
+                     int32_t use_clipped_eps, void* stream);
 /* out = c_sample*x - c_eps*(w0*e0 + w1*e1 + w2*e2 + w3*e3)    (PNDM transfer + Adams-Bashforth / RK combination;
  * unused e_i may be NULL with w_i = 0) */
 int bg_pndm_step(const float* x, float* out, int64_t n, float c_sample, float c_eps, const float* e0, float w0,

@@ -38,6 +38,10 @@ import test_gpu_sample_noise as SN   # noqa: E402
 run("keyed noise", SN.test_randn_keyed_matches_numpy_philox, 13, 1, 0)
 run("keyed steps", SN.test_keyed_step_equals_batch_step_fed_keyed_noise_and_table_form, 7, 0.6)
 run("keyed bad args", SN.test_bad_keyed_arguments_are_rejected_and_launch_nothing)
+import test_gpu_ddim as DD   # noqa: E402
+run("ddim step", DD.test_step_matches_float64, 0, 10, False, 0.5)
+run("ddim forms", DD.test_eager_keyed_and_table_forms_agree, 7, 0.6, 1)
+run("ddim bad args", DD.test_bad_arguments_are_rejected_and_launch_nothing)
 if what != "ops-no-res1":
     run("gemm", T.test_gemm, 128 * 170 + 5, 768, 1024, 0, 0, True, True, 0)   # persistent tiles wrap, residual epilogue
 if what == "all":
