@@ -257,6 +257,62 @@ __global__ void __launch_bounds__(256) ddim_step_kernel(const DdimP p) {
   }
 }
 
+// Known-token replacement (B-rep completion): x[i] = sa*known[i] + sb*z for every element of a token whose mask byte is
+// set; every other element is neither read nor written.  z: explicit `noise`, else per-sample keys (keyed_normal4, domain
+// 2, counter word t_ctr), else the batch key `seed` over the whole tensor as one sample (per_sample = n).  Groups of 4
+// never straddle two samples, as in the keyed steps.  Table form (coef != NULL): (sa, sb) from coef[*step], t_ctr from
+// *t_cur.  Traffic: the mask byte of each token, plus known (4 B) and x (4 B) per element of a known token.
+struct ReplaceP {
+  float* x;
+  const float *known, *noise;
+  const unsigned char* mask;
+  long long n, per_token, per_sample;
+  float sa, sb;
+  unsigned long long seed;
+  const unsigned long long* keys;
+  long long t;
+  const float* coef;
+  const int* step;
+  const long long* t_cur;
+};
+__global__ void __launch_bounds__(256) replace_known_kernel(const ReplaceP p) {
+  float sa = p.sa, sb = p.sb;
+  long long t = p.t;
+  if (p.coef) {
+    const float* cf = p.coef + 2 * (long long)*p.step;
+    sa = cf[0]; sb = cf[1];
+    t = *p.t_cur;
+  }
+  const long long gps = (p.per_sample + 3) / 4, ng = (p.n / p.per_sample) * gps;
+  for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += (long long)gridDim.x * blockDim.x) {
+    const long long b = g / gps, q = g - b * gps;
+    const long long base = b * p.per_sample, js0 = q * 4;
+    const int cnt = (int)min(4ll, p.per_sample - js0);
+    // tokens of the group's elements (one division per group): at most 4 mask bytes, usually 1 or 2 distinct
+    long long tok = (base + js0) / p.per_token, r = base + js0 - tok * p.per_token;
+    bool known[4] = {false, false, false, false};
+    bool any = false;
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      if (j < cnt) {
+        known[j] = p.mask[tok] != 0;
+        any |= known[j];
+        if (++r == p.per_token) { ++tok; r = 0; }
+      }
+    if (!any) continue;
+    float z[4] = {0.f, 0.f, 0.f, 0.f};
+    if (p.noise == nullptr) keyed_normal4(p.keys ? p.keys[b] : p.seed, (unsigned long long)q, (uint32_t)t, 2u, z);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if (!known[j]) continue;
+      const long long i = base + js0 + j;
+      const float kv = p.known[i];
+      // sb == 0 (the last step, abar_prev = 1): sa*kv keeps the sign of a zero, so the token ends at known bit for bit
+      p.x[i] = sb == 0.f ? sa * kv : fmaf(sa, kv, sb * (p.noise ? p.noise[i] : z[j]));
+    }
+  }
+}
+
 // one thread: k = ++(*step);  *t_cur = ts[k]   (the denoiser reads its timestep from t_cur, the step kernel reads k)
 __global__ void step_advance_kernel(const long long* __restrict__ ts, int n, int* __restrict__ step, long long* __restrict__ t_cur) {
   int k = *step + 1;
@@ -407,6 +463,41 @@ int bg_ddim_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w
   p.use_clipped_eps = use_clipped_eps != 0; p.seed = seed; p.offset = offset0; p.offset_stride = offset_stride;
   p.coef = coef_table; p.step = step; p.t_cur = reinterpret_cast<const long long*>(t_cur);
   return launch_ddim(p, sample_keys, per_sample, stream);
+}
+
+static int launch_replace(ReplaceP& p, const uint64_t* sample_keys, int64_t per_sample, void* stream) {
+  p.keys = reinterpret_cast<const unsigned long long*>(sample_keys);
+  p.per_sample = sample_keys ? per_sample : p.n;
+  replace_known_kernel<<<grid_for((p.n / p.per_sample) * ((p.per_sample + 3) / 4)), 256, 0,
+                         reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch("replace_known_kernel launch");
+}
+
+int bg_replace_known(float* x, const float* known, const uint8_t* token_mask, int64_t n, int64_t per_token,
+                     const float* noise, uint64_t seed, const uint64_t* sample_keys, int64_t per_sample, int64_t t_ctr,
+                     float sqrt_abar, float sqrt_one_minus_abar, void* stream) {
+  BG_REQUIRE(x && known && token_mask && n > 0, "replace_known: bad arguments");
+  BG_REQUIRE(per_token > 0 && n % per_token == 0, "replace_known: n must be a positive multiple of per_token");
+  BG_REQUIRE(!sample_keys || (per_sample > 0 && per_sample % per_token == 0 && n % per_sample == 0),
+             "replace_known: per_sample must be a positive multiple of per_token that divides n");
+  BG_REQUIRE(t_ctr >= 0 && t_ctr <= 0xFFFFFFFFll, "replace_known: t_ctr must be a 32-bit unsigned value");
+  ReplaceP p = {};
+  p.x = x; p.known = known; p.noise = noise; p.mask = token_mask; p.n = n; p.per_token = per_token;
+  p.sa = sqrt_abar; p.sb = sqrt_one_minus_abar; p.seed = seed; p.t = t_ctr;
+  return launch_replace(p, sample_keys, per_sample, stream);
+}
+
+int bg_replace_known_tab(float* x, const float* known, const uint8_t* token_mask, int64_t n, int64_t per_token,
+                         uint64_t seed, const uint64_t* sample_keys, int64_t per_sample, const int64_t* t_cur,
+                         const float* coef_table, const int32_t* step, void* stream) {
+  BG_REQUIRE(x && known && token_mask && n > 0 && t_cur && coef_table && step, "replace_known_tab: bad arguments");
+  BG_REQUIRE(per_token > 0 && n % per_token == 0, "replace_known_tab: n must be a positive multiple of per_token");
+  BG_REQUIRE(!sample_keys || (per_sample > 0 && per_sample % per_token == 0 && n % per_sample == 0),
+             "replace_known_tab: per_sample must be a positive multiple of per_token that divides n");
+  ReplaceP p = {};
+  p.x = x; p.known = known; p.mask = token_mask; p.n = n; p.per_token = per_token; p.seed = seed;
+  p.coef = coef_table; p.step = step; p.t_cur = reinterpret_cast<const long long*>(t_cur);
+  return launch_replace(p, sample_keys, per_sample, stream);
 }
 
 int bg_step_advance(const int64_t* timesteps, int n_steps, int32_t* step, int64_t* t_cur, void* stream) {

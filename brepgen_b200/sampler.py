@@ -16,7 +16,7 @@ no collective on the hot path; `gather_outputs` is the one optional all_gather a
 from __future__ import annotations
 
 from dataclasses import dataclass, replace
-from typing import Dict, List, Optional, Sequence
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -144,6 +144,81 @@ def check_schedule(cfg: CascadeConfig) -> None:
             raise ValueError(f"CascadeConfig.ddim_eta must be >= 0, got {cfg.ddim_eta}")
 
 
+@dataclass
+class Completion:
+    """Known parts of a B-rep for Cascade.run(known=...): sample b keeps faces 0..n_faces[b]-1 (and, when the edge fields
+    are given, their edges) and the cascade generates the rest around them.  Units are those Cascade.run returns (boxes
+    already divided by 3); rows past n_faces[b] are ignored.  K <= num_surfaces, E = num_edges.
+      n_faces (B,) ints; surfPos (B, K, 6); surfZ (B, K, 48) or None (latents generated for the known boxes);
+      edgePos (B, K, E, 6), edge_z (B, K, E, 12), edgeV (B, K, E, 6), edge_mask (B, K, E) bool (True = padded, as edgeM):
+      all four or none, and only with surfZ."""
+    n_faces: Sequence[int]
+    surfPos: torch.Tensor
+    surfZ: Optional[torch.Tensor] = None
+    edgePos: Optional[torch.Tensor] = None
+    edge_z: Optional[torch.Tensor] = None
+    edgeV: Optional[torch.Tensor] = None
+    edge_mask: Optional[torch.Tensor] = None
+
+    @staticmethod
+    def from_outputs(out: Dict[str, torch.Tensor], n_faces: Sequence[int], edges: bool = True) -> "Completion":
+        """the first n_faces[b] faces of sample b of a previous Cascade.run output (with their latents and, if `edges`,
+        their edges): regenerating everything else is run(cfg, known=Completion.from_outputs(out, n))"""
+        n = torch.as_tensor(n_faces, dtype=torch.int64).cpu().reshape(-1)
+        nv = (~out["surfMask"]).sum(1).cpu()
+        if n.numel() != nv.numel() or bool((n < 0).any()) or bool((n > nv).any()):
+            raise ValueError(f"n_faces {n.tolist()} must give 0..(valid faces) per sample; valid faces: {nv.tolist()}")
+        K = int(n.max()) if n.numel() else 0
+        cut = lambda k: out[k][:, :K].clone()
+        e = dict(edgePos=cut("edgePos"), edge_z=cut("edge_z"), edgeV=cut("edgeV"), edge_mask=cut("edgeM")) if edges else {}
+        return Completion(n_faces=n.tolist(), surfPos=cut("surfPos"), surfZ=cut("surfZ"), **e)
+
+
+def check_completion(cfg: CascadeConfig, known: Completion) -> torch.Tensor:
+    """raises on a Completion `cfg` cannot run (host checks only; Cascade.run adds the duplicate-face check on the
+    device); returns n_faces as a CPU int64 tensor"""
+    if cfg.schedule == "reference":
+        raise NotImplementedError("completion needs schedule='ddpm' or 'ddim': PNDM's Runge-Kutta steps advance from a "
+                                  "sample stored earlier (cur_sample), so known tokens cannot be replaced between them")
+    if cfg.dense_masks or cfg.ragged_masks:
+        raise ValueError("completion runs the de-duplication; dense_masks and ragged_masks are benchmark modes")
+    B, E = cfg.batch_size, cfg.num_edges
+    n = torch.as_tensor(known.n_faces, dtype=torch.int64).cpu().reshape(-1)
+    if n.numel() != B:
+        raise ValueError(f"Completion.n_faces has {n.numel()} entries for batch_size {B}")
+
+    def shape(name, t, want):
+        if t is None or tuple(t.shape) != tuple(want):
+            raise ValueError(f"Completion.{name} must have shape {tuple(want)}, got "
+                             f"{None if t is None else tuple(t.shape)}")
+    if known.surfPos is None or known.surfPos.dim() != 3:
+        raise ValueError("Completion.surfPos must be a (B, K, 6) tensor")
+    K = known.surfPos.shape[1]
+    shape("surfPos", known.surfPos, (B, K, 6))
+    if K > cfg.num_surfaces:
+        raise ValueError(f"Completion has K = {K} face slots, more than num_surfaces = {cfg.num_surfaces}")
+    if bool((n < 0).any()) or bool((n > K).any()):
+        raise ValueError(f"Completion.n_faces must lie in [0, {K}], got {n.tolist()}")
+    if known.surfZ is not None:
+        shape("surfZ", known.surfZ, (B, K, 48))
+    edge = [known.edgePos, known.edge_z, known.edgeV, known.edge_mask]
+    if any(e is not None for e in edge):
+        if not all(e is not None for e in edge):
+            raise ValueError("Completion: give edgePos, edge_z, edgeV and edge_mask together, or none of them")
+        if known.surfZ is None:
+            raise ValueError("Completion: known edges need known surface latents (surfZ)")
+        shape("edgePos", known.edgePos, (B, K, E, 6))
+        shape("edge_z", known.edge_z, (B, K, E, 12))
+        shape("edgeV", known.edgeV, (B, K, E, 6))
+        shape("edge_mask", known.edge_mask, (B, K, E))
+        if known.edge_mask.dtype != torch.bool:
+            raise ValueError("Completion.edge_mask must be a bool tensor (True = padded)")
+        faces = torch.arange(K)[None, :] < n[:, None]
+        if bool((known.edge_mask[..., 0].cpu() & faces).any()):
+            raise ValueError("Completion.edge_mask[..., 0] is set on a known face: edge slot 0 of a face is always valid")
+    return n
+
+
 def randn_keyed(seeds: Sequence[int], stage: int, shape, device, domain: int = 1, t: int = 0) -> torch.Tensor:
     """(len(seeds), *shape[1:]) fp32 normals from the per-sample streams (bg_randn_keyed); default domain 1 = initial noise"""
     B = len(seeds)
@@ -203,13 +278,14 @@ class Cascade:
         # a forward is ~105 launches from Python (~1 ms of host time); below ~100 k tokens the GPU finishes sooner than that
         return n_steps >= 32 and tokens <= 100_000
 
-    def _loop_graph(self, cfg: CascadeConfig, sched, timesteps, x, fwd):
+    def _loop_graph(self, cfg: CascadeConfig, sched, timesteps, x, fwd, known=None):
         """sched: self.ddpm or self.ddim; timesteps: 1-D int64 CPU tensor; x: (B, ...) fp32 on the device; fwd(x_in, t_dev)
         -> eps of a (possibly CFG-doubled) batch.  The loop body of sample.py:145-153 -- [step counter / timestep advance] ->
         forward -> fused scheduler step (CFG combine, x0, clip, DDPM posterior mean or DDIM update, Philox noise) -- is
         captured ONCE and replayed len(timesteps) times: no per-step host work.  Nothing step-specific is a kernel argument:
         the timestep comes from a device scalar, the coefficients from a device table indexed by a device counter
-        (bg_step_advance / bg_ddpm_step_tab / bg_ddim_step_tab)."""
+        (bg_step_advance / bg_ddpm_step_tab / bg_ddim_step_tab).  known: {slots: (values, token mask)} of a completion;
+        bg_replace_known_tab then follows the step inside the captured body."""
         dev = self.device
         lib = _ffi.lib()
         T = len(timesteps)
@@ -228,6 +304,16 @@ class Cascade:
         else:
             seed, off0, stride = sched.philox_stream(n)
         clip = float(sched.config.clip_sample_range) if sched.config.clip_sample else 0.0
+        if known is not None:
+            kn, km = known[xb.shape[1]]
+            rtab = sched.replace_table(timesteps).to(dev)
+            rseed = 0 if keyed else sched.replace_seed()
+
+        def replace(st):
+            if known is not None:
+                _ffi.check(lib.bg_replace_known_tab(xb.data_ptr(), kn.data_ptr(), km.data_ptr(), n, xb.shape[-1], rseed,
+                                                    _ffi.ptr(keys), n // B, t_cur.data_ptr(), rtab.data_ptr(),
+                                                    step.data_ptr(), st), "bg_replace_known_tab")
 
         def body():
             st = _ffi.current_stream()
@@ -239,15 +325,15 @@ class Cascade:
                 _ffi.check(lib.bg_ddim_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(),
                                                 xb.data_ptr(), seed, off0, stride, _ffi.ptr(keys), n // B, t_cur.data_ptr(),
                                                 n, coef.data_ptr(), step.data_ptr(), clip, 0, st), "bg_ddim_step_tab")
-                return
-            if keyed:
+            elif keyed:
                 _ffi.check(lib.bg_ddpm_step_tab_keyed(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(),
                                                       xb.data_ptr(), keys.data_ptr(), n // B, t_cur.data_ptr(), n,
                                                       coef.data_ptr(), step.data_ptr(), clip, st), "bg_ddpm_step_tab_keyed")
-                return
-            _ffi.check(lib.bg_ddpm_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(), xb.data_ptr(),
-                                            seed, off0, stride, n, coef.data_ptr(), step.data_ptr(), clip, st),
-                       "bg_ddpm_step_tab")
+            else:
+                _ffi.check(lib.bg_ddpm_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(),
+                                                xb.data_ptr(), seed, off0, stride, n, coef.data_ptr(), step.data_ptr(), clip,
+                                                st), "bg_ddpm_step_tab")
+            replace(st)
 
         # warm-up outside the capture (packs the weights, allocates the workspace), then rewind the state it touched
         x0 = xb.clone()
@@ -272,12 +358,17 @@ class Cascade:
         return xb
 
     # ------------------------------------------------------------------ one denoising loop
-    def _loop(self, cfg: CascadeConfig, sched, timesteps, x, fwd, label2, gen, on_step=None, noise_fn=None):
-        """fwd(x_in, t_dev) -> eps for a (possibly CFG-doubled) batch; noise_fn(k, shape) -> explicit DDPM / DDIM step noise"""
+    def _loop(self, cfg: CascadeConfig, sched, timesteps, x, fwd, label2, gen, on_step=None, noise_fn=None, known=None,
+              rnoise_fn=None):
+        """fwd(x_in, t_dev) -> eps for a (possibly CFG-doubled) batch; noise_fn(k, shape) -> explicit DDPM / DDIM step noise.
+        known: {slots: (values, token mask)} of a completion: the known tokens are replaced before the first step and after
+        every step (sched.replace_known); rnoise_fn(k, shape) -> explicit replacement noise (k = -1 before the first step)."""
         B = x.shape[0]
         k = 0
         fused = isinstance(sched, (DDPMScheduler, DDIMScheduler))    # CFG combine and noise inside the step kernel
-        if fused and noise_fn is None and gen is None and len(timesteps) > 0 and \
+        if known is not None and len(timesteps) > 0:
+            x = self._replace(sched, known, x, timesteps[0], -1, rnoise_fn, initial=True)
+        if fused and noise_fn is None and rnoise_fn is None and gen is None and len(timesteps) > 0 and \
                 self._use_graph(cfg, len(timesteps), x[0].numel() // x.shape[-1] * B * (2 if cfg.use_cf else 1)):
             # on_step (the late face-count increase, sample.py:140-142) changes the shape once: one graph per segment
             lo = 0
@@ -291,7 +382,7 @@ class Cascade:
                         hi += 1
                 else:
                     hi = len(ts_list)
-                x = self._loop_graph(cfg, sched, timesteps[lo:hi], x, fwd)
+                x = self._loop_graph(cfg, sched, timesteps[lo:hi], x, fwd, known)
                 lo = hi
             return x
         ts_dev = timesteps.to(self.device)
@@ -318,8 +409,17 @@ class Cascade:
                     x = self._fused_step(cfg, sched, k, t, x, pred, gen, noise_fn)
                 else:
                     x = sched.step(pred, t, x).prev_sample
+            if known is not None:
+                x = self._replace(sched, known, x, t, k, rnoise_fn)
             k += 1
         return x
+
+    def _replace(self, sched, known, x, t, k, rnoise_fn, initial=False):
+        """known tokens of x noised to the level step k at t left it at (initial: the stage's starting level); in place on
+        a step's output, on a copy of the stage's initial noise (which may be the caller's init_noise tensor)"""
+        kn, km = known[x.shape[1]]
+        nz = rnoise_fn(k, x.shape).to(self.device) if rnoise_fn is not None else None
+        return sched.replace_known(x, kn, km, t, noise=nz, out=None if initial else x, initial=initial)
 
     def _fused_step(self, cfg, sched, k, t, x, pred, gen, noise_fn, **cf):
         """one DDPM or DDIM step; explicit noise from noise_fn on the steps where diffusers draws it: DDPM at t > 0, DDIM
@@ -332,7 +432,8 @@ class Cascade:
 
     _STAGE_ID = {"surfPos": 0, "surfZ": 1, "edgePos": 2, "edgeZV": 3}
 
-    def _stage(self, cfg, x, fwd, label2, gen, hybrid_ddpm_tail: bool, on_step=None, noise_fn=None, name="surfPos"):
+    def _stage(self, cfg, x, fwd, label2, gen, hybrid_ddpm_tail: bool, on_step=None, noise_fn=None, name="surfPos",
+               known=None, rnoise_fn=None):
         seeds = getattr(self, "_sample_seeds", None)
         noisy = self.ddim if cfg.schedule == "ddim" else self.ddpm
         if seeds is not None:
@@ -341,10 +442,10 @@ class Cascade:
             noisy.set_noise_seed(*getattr(self, "_noise_key", (int(cfg.seed), 0)), self._STAGE_ID[name])
         if cfg.schedule == "ddim":
             self.ddim.set_timesteps(cfg.ddim_steps)
-            return self._loop(cfg, self.ddim, self.ddim.timesteps, x, fwd, label2, gen, on_step, noise_fn)
+            return self._loop(cfg, self.ddim, self.ddim.timesteps, x, fwd, label2, gen, on_step, noise_fn, known, rnoise_fn)
         if cfg.schedule == "ddpm":
             self.ddpm.set_timesteps(cfg.ddpm_steps)
-            return self._loop(cfg, self.ddpm, self.ddpm.timesteps, x, fwd, label2, gen, on_step, noise_fn)
+            return self._loop(cfg, self.ddpm, self.ddpm.timesteps, x, fwd, label2, gen, on_step, noise_fn, known, rnoise_fn)
         # the shipped hybrid: PNDM(200) then, for the position stages, DDPM(1000)[-250:]
         self.pndm.set_timesteps(200)
         ts = self.pndm.timesteps[:158] if hybrid_ddpm_tail else self.pndm.timesteps
@@ -356,15 +457,65 @@ class Cascade:
             x = self._loop(cfg, self.ddpm, self.ddpm.timesteps[-250:], x, fwd, label2, gen, None, noise_fn)
         return x
 
+    # ------------------------------------------------------------------ completion
+    def _known_tensors(self, cfg: CascadeConfig, known: Completion, n: torch.Tensor) -> dict:
+        """device tensors of a checked Completion: per stage {slots: (model-unit values, uint8 token mask)}, plus the face
+        mask 'face' (B, S), the given edge masks 'edgeM' and the given outputs 'out' to write through.  Raises ValueError
+        when known faces of a sample duplicate each other under the de-duplication rule (bg_dedup_surfaces on the
+        model-unit boxes): the de-duplication would then drop a known face."""
+        dev = self.device
+        B, S0, E = cfg.batch_size, cfg.num_surfaces, cfg.num_edges
+        S = S0 if cfg.use_cf else 2 * S0
+        K = known.surfPos.shape[1]
+        nd = n.to(dev)
+        f32 = lambda t: t.to(device=dev, dtype=torch.float32).contiguous()
+
+        def pad(t, slots):            # (B, K, ...) -> (B, slots, ...), zero past K
+            p = torch.zeros((B, slots) + tuple(t.shape[2:]), dtype=t.dtype, device=dev)
+            p[:, :K] = t.to(dev)
+            return p
+        face = lambda slots: torch.arange(slots, device=dev)[None, :] < nd[:, None]
+        pos = f32(known.surfPos) * 3.0
+        if K > 0 and bool((n > 1).any()):
+            rows = torch.where(face(K)[..., None], pos, pos[:, :1])    # past n_faces: copies of face 0, always dropped
+            _, m = dedup_surfaces(rows, cfg.bbox_threshold)
+            bad = (m & face(K)).any(1).cpu()
+            if bool(bad.any()):
+                raise ValueError(f"Completion: known faces of samples {torch.nonzero(bad).flatten().tolist()} duplicate "
+                                 f"each other under the de-duplication rule (bbox_threshold {cfg.bbox_threshold})")
+        u8 = lambda m: m.to(torch.uint8).contiguous()
+        kn = {"face": face(S), "out": {"surfPos": pad(f32(known.surfPos), S)}}
+        kn["surfPos"] = {S0: (pad(pos, S0), u8(face(S0)))}
+        if not cfg.use_cf:            # the late increase doubles the slots: both copies stay known
+            kn["surfPos"][2 * S0] = (pad(pos, S0).repeat(1, 2, 1), u8(face(S0).repeat(1, 2)))
+        if known.surfZ is not None:
+            kn["surfZ"] = {S: (pad(f32(known.surfZ), S), u8(face(S)))}
+            kn["out"]["surfZ"] = kn["surfZ"][S][0]
+        if known.edgePos is not None:
+            em = u8(face(S)[..., None].expand(B, S, E))
+            kn["edgePos"] = {S: (pad(f32(known.edgePos) * 3.0, S), em)}
+            zv = torch.cat([f32(known.edge_z), f32(known.edgeV)], -1)
+            kn["edgeZV"] = {S: (pad(zv, S), em)}
+            kn["edgeM"] = pad(known.edge_mask.to(torch.bool), S)
+            kn["out"].update(edgePos=pad(f32(known.edgePos), S), edgeM=kn["edgeM"], edge_z=pad(f32(known.edge_z), S),
+                             edgeV=pad(f32(known.edgeV), S))
+        return kn
+
     # ------------------------------------------------------------------ the cascade
     @torch.no_grad()
-    def run(self, cfg: CascadeConfig, init_noise: Optional[Dict[str, torch.Tensor]] = None, step_noise=None):
+    def run(self, cfg: CascadeConfig, init_noise: Optional[Dict[str, torch.Tensor]] = None, step_noise=None,
+            known: Optional[Completion] = None, replace_noise=None):
         """step_noise(stage_name, k, shape) -> tensor: explicit DDPM / DDIM step noise of step k (parity runs; DDPM draws it
         at t > 0, DDIM on every step when ddim_eta > 0); default = in-kernel Philox
         keyed by (cfg.seed, rank, stage): reproducible from cfg.seed, independent across ranks and stages.
         cfg.noise == "per_sample": initial and step noise come from each sample's own streams (bg_randn_keyed and the keyed
-        step kernels), so sample b's outputs depend on its seed alone; init_noise / step_noise still take precedence."""
+        step kernels), so sample b's outputs depend on its seed alone; init_noise / step_noise still take precedence.
+        known: a Completion (schedules "ddpm" and "ddim"): every stage that has known tokens replaces them before its
+        first step and after every step with the known values noised to the step's level, so the rest is generated
+        around them; the known parts come out as given, bit for bit.  replace_noise(stage_name, k, shape) -> tensor:
+        explicit noise of that replacement (k = -1 before the first step; parity runs), mirroring step_noise."""
         check_schedule(cfg)
+        n_known = check_completion(cfg, known) if known is not None else None
         seeds = per_sample_seeds(cfg)
         self._sample_seeds = seeds
         dev = self.device
@@ -377,9 +528,12 @@ class Cascade:
             pass
         self._noise_key = (int(cfg.seed), rank)
         nf = (lambda name: (lambda k, shape: step_noise(name, k, shape))) if step_noise is not None else (lambda name: None)
+        rnf = (lambda name: (lambda k, shape: replace_noise(name, k, shape))) if replace_noise is not None else \
+            (lambda name: None)
         gen = None
         B, S0, E = cfg.batch_size, cfg.num_surfaces, cfg.num_edges
         S = S0 if cfg.use_cf else 2 * S0
+        kn = self._known_tensors(cfg, known, n_known) if known is not None else {}
         cpu_gen = torch.Generator().manual_seed(cfg.seed)             # initial noise: CPU generator (utils.py:62-97)
         label2 = None
         if cfg.use_cf:
@@ -404,7 +558,8 @@ class Cascade:
 
         surfPos = noise("surfPos", (B, S0, 6))
         surfPos = self._stage(cfg, surfPos, lambda x, t: self.m["surfpos"](x, t, label2), label2, gen, True,
-                              on_step=late_increase, noise_fn=nf("surfPos"), name="surfPos")
+                              on_step=late_increase, noise_fn=nf("surfPos"), name="surfPos", known=kn.get("surfPos"),
+                              rnoise_fn=rnf("surfPos"))
         if not cfg.use_cf and surfPos.shape[1] == S0:
             surfPos = surfPos.repeat(1, 2, 1)
 
@@ -422,13 +577,13 @@ class Cascade:
         # STEP 1-3 surface latents (sample.py:189-202)
         surfZ = noise("surfZ", (B, S, 48))
         surfZ = self._stage(cfg, surfZ, lambda x, t: self.m["surfz"](x, t, sP, sM, label2), label2, gen, False,
-                            noise_fn=nf("surfZ"), name="surfZ")
+                            noise_fn=nf("surfZ"), name="surfZ", known=kn.get("surfZ"), rnoise_fn=rnf("surfZ"))
         sZ = rep2(surfZ)
 
         # STEP 2-1 edge positions (sample.py:208-236)
         edgePos = noise("edgePos", (B, S, E, 6))
         edgePos = self._stage(cfg, edgePos, lambda x, t: self.m["edgepos"](x, t, sP, sZ, sM, label2), label2, gen, True,
-                              noise_fn=nf("edgePos"), name="edgePos")
+                              noise_fn=nf("edgePos"), name="edgePos", known=kn.get("edgePos"), rnoise_fn=rnf("edgePos"))
 
         # STEP 2-2 duplicate edges per face (sample.py:242-261)
         if cfg.ragged_masks:
@@ -438,17 +593,24 @@ class Cascade:
             edgeM = torch.zeros(B, S, E, dtype=torch.bool, device=dev)
         else:
             edgeM = dedup_edges(edgePos, surfMask, cfg.bbox_threshold)
+        if "edgeM" in kn:             # the known faces keep their given edge masks
+            edgeM = torch.where(kn["face"][..., None], kn["edgeM"], edgeM)
         eP, eM = rep2(edgePos), rep2(edgeM)
 
         # STEP 2-3 edge latents + vertices (sample.py:267-286)
         edgeZV = noise("edgeZV", (B, S, E, 18))
         edgeZV = self._stage(cfg, edgeZV, lambda x, t: self.m["edgez"](x, t, eP, sP, sZ, eM, label2), label2, gen, False,
-                             noise_fn=nf("edgeZV"), name="edgeZV")
+                             noise_fn=nf("edgeZV"), name="edgeZV", known=kn.get("edgeZV"), rnoise_fn=rnf("edgeZV"))
         edgeZV = edgeZV.masked_fill(edgeM.unsqueeze(-1), 0.0)
         edge_z, edgeV = edgeZV[..., :12], edgeZV[..., 12:]
 
         out = {"surfPos": surfPos / 3.0, "surfMask": surfMask, "surfZ": surfZ, "edgePos": edgePos / 3.0, "edgeM": edgeM,
                "edge_z": edge_z.contiguous(), "edgeV": edgeV.contiguous()}
+        if kn:                        # the given values of the known faces, written through (the decoders see them too)
+            for k, v in kn["out"].items():
+                f = kn["face"].reshape(kn["face"].shape + (1,) * (v.dim() - 2))
+                out[k] = torch.where(f, v, out[k]).contiguous()
+            surfZ, edge_z = out["surfZ"], out["edge_z"]
         # decoders (sample.py:289-294)
         if cfg.decode and self.surf_vae is not None:
             z = surfZ.unflatten(-1, (16, 3)).flatten(0, 1).permute(0, 2, 1).unflatten(-1, (4, 4))

@@ -165,6 +165,74 @@ class _NoiseStreams:
     def advance_philox(self, n: int, steps: int):
         self._philox_offset += steps * ((n + 3) // 4)
 
+    # ---------------------------------------------------------------- known-token replacement (B-rep completion)
+    def _abar_prev(self, t: int) -> torch.Tensor:
+        raise NotImplementedError
+
+    def replace_coefficients(self, t: int, initial: bool = False):
+        """(sqrt(abar), sqrt(1 - abar)) as Python floats (fp32 arithmetic): abar = abar_prev(t) of this scheduler's step
+        convention, the noise level `step` leaves x at; initial=True: abar_t itself, the level of a stage's starting noise"""
+        a = self.alphas_cumprod[int(t)] if initial else self._abar_prev(int(t))
+        return float(a ** 0.5), float((1 - a) ** 0.5)
+
+    def replace_table(self, timesteps) -> torch.Tensor:
+        """[len(timesteps), 2] fp32 (CPU): replace_coefficients(t) for every t of a denoising loop -- the device table that
+        bg_replace_known_tab indexes with the step counter of bg_step_advance"""
+        rows = [self.replace_coefficients(_as_int(t)) for t in timesteps]
+        return torch.tensor(rows, dtype=torch.float32).reshape(-1, 2)
+
+    def replace_seed(self) -> int:
+        """batch-mode key of the replacement noise: mix_seed(step stream key, 2).  Reads the step stream's key but never
+        its offset, so replacing tokens leaves the step noise exactly as it is without replacement."""
+        if self._philox_seed is None:
+            self._philox_seed = mix_seed(torch.initial_seed())
+        return mix_seed(self._philox_seed, 2)
+
+    def replace_known(self, sample: torch.Tensor, known: torch.Tensor, known_mask: torch.Tensor, timestep,
+                      noise: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None, initial: bool = False):
+        """The sample with its known tokens set to q(x_prev(t) | known) = sqrt(abar_prev) known + sqrt(1 - abar_prev) z
+        (inpainting by replacement): call it after `step(..., t, ...)` with the same t.  A token is the last dimension:
+        known_mask has sample.shape[:-1], True = known; other tokens are left bit for bit as they are.  z: `noise`, else
+        the per-sample streams of set_sample_keys (domain 2, counter t), else the batch key replace_seed() (counter t),
+        which does not move the step's noise stream.  initial=True: the replacement before the first step at t (noise
+        level abar_t, counter t + 1).  out: destination, may be `sample` (in place); default a new tensor."""
+        if tuple(known.shape) != tuple(sample.shape) or tuple(known_mask.shape) != tuple(sample.shape[:-1]):
+            raise RuntimeError(f"replace_known: known {tuple(known.shape)} and known_mask {tuple(known_mask.shape)} must "
+                               f"have the sample's shape {tuple(sample.shape)} and its shape without the last dimension")
+        if noise is not None and tuple(noise.shape) != tuple(sample.shape):
+            raise RuntimeError(f"replace_known: noise has shape {tuple(noise.shape)}, sample has {tuple(sample.shape)}")
+        if out is not None and (out.dtype != torch.float32 or not out.is_contiguous() or out.device != sample.device or
+                                tuple(out.shape) != tuple(sample.shape)):
+            raise RuntimeError("replace_known: `out` must be a contiguous fp32 tensor of the sample's shape and device")
+        _require_cuda(sample, "sample")
+        t = _as_int(timestep)
+        sa, sb = self.replace_coefficients(t, initial)
+        t_ctr = t + 1 if initial else t
+        if out is None:
+            dst = sample.float().contiguous().clone()
+        else:
+            dst = out
+            if dst.data_ptr() != sample.data_ptr():
+                dst.copy_(sample)
+        kn = known.to(device=dst.device, dtype=torch.float32).contiguous()
+        m = known_mask.to(device=dst.device, dtype=torch.uint8).contiguous()
+        if noise is not None:
+            noise = noise.to(device=dst.device, dtype=torch.float32).contiguous()
+        n = dst.numel()
+        seed, keys = 0, None
+        if noise is None:
+            if self._sample_seeds is not None:
+                keys = self.sample_key_tensor(dst.shape[0], dst.device)
+            else:
+                seed = self.replace_seed()
+        if n == 0:
+            return dst
+        with torch.cuda.device(dst.device):
+            _ffi.check(_ffi.lib().bg_replace_known(dst.data_ptr(), kn.data_ptr(), m.data_ptr(), n, dst.shape[-1],
+                                                  _ffi.ptr(noise), seed, _ffi.ptr(keys), n // dst.shape[0], t_ctr, sa, sb,
+                                                  _ffi.current_stream()), "bg_replace_known")
+        return dst
+
 
 class DDPMScheduler(_NoiseStreams):
     def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.0001, beta_end: float = 0.02,
@@ -210,6 +278,10 @@ class DDPMScheduler(_NoiseStreams):
         if t > 0:
             sigma = float(torch.clamp(b_prev / b_t * cur_beta, min=1e-20) ** 0.5)
         return float(b_t ** 0.5), float(a_t ** 0.5), float(c_x0), float(c_x), sigma
+
+    def _abar_prev(self, t: int) -> torch.Tensor:
+        prev_t = t - self.config.num_train_timesteps // self.num_inference_steps
+        return self.alphas_cumprod[prev_t] if prev_t >= 0 else self.one
 
     def coefficient_table(self, timesteps) -> torch.Tensor:
         """[len(timesteps), 5] fp32 (CPU): step_coefficients(t) for every t of a denoising loop -- the device table that
@@ -324,6 +396,13 @@ class DDIMScheduler(_NoiseStreams):
         std_dev_t = eta * variance ** 0.5
         c_dir = (1 - a_prev - std_dev_t ** 2) ** 0.5
         return float(b_t ** 0.5), float(a_t ** 0.5), float(a_prev ** 0.5), float(c_dir), float(std_dev_t)
+
+    def _abar_prev(self, t: int) -> torch.Tensor:
+        if self.num_inference_steps is None:
+            raise ValueError("Number of inference steps is 'None', you need to run 'set_timesteps' after creating the "
+                             "scheduler")
+        prev_t = t - self.config.num_train_timesteps // self.num_inference_steps
+        return self.alphas_cumprod[prev_t] if prev_t >= 0 else self.final_alpha_cumprod
 
     def coefficient_table(self, timesteps, eta: float = 0.0) -> torch.Tensor:
         """[len(timesteps), 5] fp32 (CPU): step_coefficients(t, eta) for every t of a denoising loop -- the device table

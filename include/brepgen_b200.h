@@ -156,7 +156,8 @@ int bg_step_advance(const int64_t* timesteps, int n_steps, int32_t* step, int64_
 /* Per-sample noise streams (opt-in; the functions above keep the batch-wide (seed, offset) stream).  sample_keys: device
  * uint64 [n_samples], one Philox4x32-10 key per sample.  Element j of sample b is normal (j % 4) of the block with key
  * sample_keys[b] and counter (j / 4 as 64 bits, t, domain), Box-Muller as bg_ddpm_step; a block of 4 never straddles two
- * samples.  domain 0 = DDPM step noise at timestep t, domain 1 = initial noise (t = 0).  A sample's noise is therefore a
+ * samples.  domain 0 = DDPM step noise at timestep t, domain 1 = initial noise (t = 0), domain 2 = known-token
+ * replacement noise (bg_replace_known; t = the counter word t_ctr).  A sample's noise is therefore a
  * function of its key alone, whatever the batch size, its position in the batch or the rank that runs it.
  * NULL sample_keys, per_sample <= 0 or n not a multiple of per_sample: BG_STATUS_BAD_ARG, nothing is launched. */
 /* out[b * per_sample + j] = normal j of sample b  (n_samples * per_sample fp32) */
@@ -195,6 +196,26 @@ int bg_ddim_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w
                      uint64_t offset0, uint64_t offset_stride, const uint64_t* sample_keys, int64_t per_sample,
                      const int64_t* t_cur, int64_t n, const float* coef_table, const int32_t* step, float clip,
                      int32_t use_clipped_eps, void* stream);
+/* Known-token replacement (B-rep completion; runs after the step kernel, in place on x).  x is n fp32 elements in tokens
+ * of per_token consecutive elements; token_mask holds one byte per token (n / per_token).  For every element of a token
+ * whose byte is non-zero:  x[i] = sqrt_abar*known[i] + sqrt_one_minus_abar*z  (fmaf(sa, known, sb*z); sa*known when
+ * sb == 0, so a last step with abar_prev = 1 ends at known bit for bit).  Every other element is neither read nor written.
+ * z: the explicit `noise` tensor if not NULL; else, when sample_keys != NULL, normal (j % 4) of the per-sample stream of
+ * sample b = i / per_sample at counter (j / 4, t_ctr, domain 2), j = i % per_sample (bg_randn_keyed(domain 2, t_ctr));
+ * else the batch key `seed`, the whole tensor counted as one sample: counter (i / 4, t_ctr, 2).  The batch form draws
+ * from its own key and domain, so it neither reads nor advances the (seed, offset) stream of the step kernels.
+ * t_ctr: the timestep t of the step just taken, or t_first + 1 for the replacement before a stage's first step.
+ * NULL x / known / token_mask, n <= 0, per_token <= 0, n not a multiple of per_token, (keyed) per_sample not a positive
+ * multiple of per_token or not dividing n, t_ctr outside 32 bits: BG_STATUS_BAD_ARG, nothing is launched. */
+int bg_replace_known(float* x, const float* known, const uint8_t* token_mask, int64_t n, int64_t per_token,
+                     const float* noise, uint64_t seed, const uint64_t* sample_keys, int64_t per_sample, int64_t t_ctr,
+                     float sqrt_abar, float sqrt_one_minus_abar, void* stream);
+/* table-driven form for graph capture: coef_table[k][2] = (sqrt(abar_prev), sqrt(1-abar_prev)) of step k = *step
+ * (bg_step_advance) and t_ctr = *t_cur; no explicit noise.  Bit-identical to bg_replace_known with the same coefficients,
+ * t_ctr and keys or seed.  NULL t_cur / coef_table / step are BG_STATUS_BAD_ARG too. */
+int bg_replace_known_tab(float* x, const float* known, const uint8_t* token_mask, int64_t n, int64_t per_token,
+                         uint64_t seed, const uint64_t* sample_keys, int64_t per_sample, const int64_t* t_cur,
+                         const float* coef_table, const int32_t* step, void* stream);
 /* out = c_sample*x - c_eps*(w0*e0 + w1*e1 + w2*e2 + w3*e3)    (PNDM transfer + Adams-Bashforth / RK combination;
  * unused e_i may be NULL with w_i = 0) */
 int bg_pndm_step(const float* x, float* out, int64_t n, float c_sample, float c_eps, const float* e0, float w0,

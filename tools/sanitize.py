@@ -42,6 +42,10 @@ import test_gpu_ddim as DD   # noqa: E402
 run("ddim step", DD.test_step_matches_float64, 0, 10, False, 0.5)
 run("ddim forms", DD.test_eager_keyed_and_table_forms_agree, 7, 0.6, 1)
 run("ddim bad args", DD.test_bad_arguments_are_rejected_and_launch_nothing)
+import test_gpu_completion as CO   # noqa: E402
+run("replace known", CO.test_kernel_matches_float64, 18, 13, "random")
+run("replace forms", CO.test_noise_forms_agree, 6, 7)
+run("replace bad args", CO.test_bad_arguments_are_rejected_and_launch_nothing)
 if what != "ops-no-res1":
     run("gemm", T.test_gemm, 128 * 170 + 5, 768, 1024, 0, 0, True, True, 0)   # persistent tiles wrap, residual epilogue
 if what == "all":
