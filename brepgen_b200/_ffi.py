@@ -52,6 +52,9 @@ SIGNATURES = {
     "bg_ddpm_step_tab_keyed": (i32, [vp, vp, f32, vp, vp, vp, i64, vp, i64, vp, vp, f32, vp]),
     "bg_ddim_step": (i32, [vp, vp, f32, vp, vp, vp, u64, u64, vp, i64, i64, i64, f32, f32, f32, f32, f32, f32, i32, vp]),
     "bg_ddim_step_tab": (i32, [vp, vp, f32, vp, vp, u64, u64, u64, vp, i64, vp, i64, vp, vp, f32, i32, vp]),
+    "bg_dpm_step": (i32, [vp, vp, f32, vp, vp, vp, vp, u64, u64, vp, i64, i64, i64, f32, f32, f32, f32, f32, f32, f32, f32,
+                          vp]),
+    "bg_dpm_step_tab": (i32, [vp, vp, f32, vp, vp, vp, u64, u64, u64, vp, i64, vp, i64, vp, vp, f32, vp]),
     "bg_replace_known": (i32, [vp, vp, vp, i64, i64, vp, u64, vp, i64, i64, f32, f32, vp]),
     "bg_replace_known_tab": (i32, [vp, vp, vp, i64, i64, u64, vp, i64, vp, vp, vp, vp]),
     "bg_pndm_step": (i32, [vp, vp, i64, f32, f32, vp, f32, vp, f32, vp, f32, vp, f32, vp]),

@@ -257,6 +257,82 @@ __global__ void __launch_bounds__(256) ddim_step_kernel(const DdimP p) {
   }
 }
 
+// DPM-Solver++ multistep step (diffusers 0.27 DPMSolverMultistepScheduler, epsilon prediction, midpoint), first or second
+// order, ODE ("dpmsolver++", c_z = 0) or SDE ("sde-dpmsolver++"):
+//   x0 = (x - sigma_s*e) / alpha_s, clamped to +-clip;  m1 = hist[i];  hist[i] = x0;  D1 = (x0 - m1) * inv_r0;
+//   out = c_x*x + c_0*x0 + c_1*D1 + c_z*z.
+// Every product and sum is rounded on its own, in diffusers' order (D1 first, then the sum left to right), so the step
+// tracks the fp32 torch oracle rather than an FMA-contracted variant of it.  c_1 == 0 (a first-order step) never reads
+// hist; hist == NULL skips the store.  hist[i] is read and written by the thread that owns element i, so the update is
+// in place.  Noise (only when c_z != 0) and the table form (coefficients from coef[7 * *step], t from *t_cur, batch offset
+// offset + k * offset_stride) as ddim_step_kernel.
+struct DpmP {
+  const float *eps_c, *eps_u, *x, *noise;
+  float *out, *hist;
+  long long n, per_sample;
+  float w, alpha_s, sigma_s, c_x, c_0, c_1, inv_r0, c_z, clip;
+  const unsigned long long* keys;
+  long long t;
+  unsigned long long seed, offset, offset_stride;
+  const float* coef;
+  const int* step;
+  const long long* t_cur;
+};
+__global__ void __launch_bounds__(256) dpm_step_kernel(const DpmP p) {
+  float alpha_s = p.alpha_s, sigma_s = p.sigma_s, c_x = p.c_x, c_0 = p.c_0, c_1 = p.c_1, inv_r0 = p.inv_r0, c_z = p.c_z;
+  long long t = p.t;
+  unsigned long long offset = p.offset;
+  if (p.coef) {
+    const int k = *p.step;
+    const float* cf = p.coef + 7 * (long long)k;
+    alpha_s = cf[0]; sigma_s = cf[1]; c_x = cf[2]; c_0 = cf[3]; c_1 = cf[4]; inv_r0 = cf[5]; c_z = cf[6];
+    if (p.t_cur) t = *p.t_cur;
+    offset += (unsigned long long)k * p.offset_stride;
+  }
+  const long long gps = (p.per_sample + 3) / 4, ng = (p.n / p.per_sample) * gps;
+  for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += (long long)gridDim.x * blockDim.x) {
+    const long long b = g / gps, q = g - b * gps;
+    float z[4] = {0.f, 0.f, 0.f, 0.f};
+    if (c_z != 0.f && p.noise == nullptr) {
+      if (p.keys) {
+        keyed_normal4(p.keys[b], (unsigned long long)q, (uint32_t)t, 0u, z);
+      } else {
+        uint32_t r[4];
+        const unsigned long long ctr = offset + (unsigned long long)q;
+        philox4x32_10((uint32_t)ctr, (uint32_t)(ctr >> 32), 0u, 0u, (uint32_t)p.seed, (uint32_t)(p.seed >> 32), r);
+        box_muller(r[0], r[1], z[0], z[1]);
+        box_muller(r[2], r[3], z[2], z[3]);
+      }
+    }
+    // the group's loads first, then the math and the stores: no load waits behind a store it might alias
+    const long long i0 = b * p.per_sample + q * 4;
+    const int cnt = (int)min(4ll, p.per_sample - q * 4);
+    float e[4], xv[4], m1[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if (j < cnt) {
+        e[j] = p.eps_c[i0 + j];
+        if (p.eps_u) e[j] = __fsub_rn(__fmul_rn(e[j], 1.f + p.w), __fmul_rn(p.eps_u[i0 + j], p.w));
+        xv[j] = p.x[i0 + j];
+        if (c_1 != 0.f) m1[j] = p.hist[i0 + j];
+        if (c_z != 0.f && p.noise) z[j] = p.noise[i0 + j];
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if (j < cnt) {
+        float x0 = __fdiv_rn(__fsub_rn(xv[j], __fmul_rn(sigma_s, e[j])), alpha_s);
+        if (p.clip > 0.f) x0 = fminf(fmaxf(x0, -p.clip), p.clip);
+        float o = __fadd_rn(__fmul_rn(c_x, xv[j]), __fmul_rn(c_0, x0));
+        if (c_1 != 0.f) o = __fadd_rn(o, __fmul_rn(c_1, __fmul_rn(__fsub_rn(x0, m1[j]), inv_r0)));
+        if (c_z != 0.f) o = __fadd_rn(o, __fmul_rn(c_z, z[j]));
+        if (p.hist) p.hist[i0 + j] = x0;
+        p.out[i0 + j] = o;
+      }
+    }
+  }
+}
+
 // Known-token replacement (B-rep completion): x[i] = sa*known[i] + sb*z for every element of a token whose mask byte is
 // set; every other element is neither read nor written.  z: explicit `noise`, else per-sample keys (keyed_normal4, domain
 // 2, counter word t_ctr), else the batch key `seed` over the whole tensor as one sample (per_sample = n).  Groups of 4
@@ -463,6 +539,44 @@ int bg_ddim_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w
   p.use_clipped_eps = use_clipped_eps != 0; p.seed = seed; p.offset = offset0; p.offset_stride = offset_stride;
   p.coef = coef_table; p.step = step; p.t_cur = reinterpret_cast<const long long*>(t_cur);
   return launch_ddim(p, sample_keys, per_sample, stream);
+}
+
+static int launch_dpm(DpmP& p, const uint64_t* sample_keys, int64_t per_sample, void* stream) {
+  p.keys = reinterpret_cast<const unsigned long long*>(sample_keys);
+  p.per_sample = sample_keys ? per_sample : p.n;
+  dpm_step_kernel<<<grid_for((p.n / p.per_sample) * ((p.per_sample + 3) / 4)), 256, 0,
+                    reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch("dpm_step_kernel launch");
+}
+
+int bg_dpm_step(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out, float* hist,
+                const float* noise, uint64_t seed, uint64_t offset, const uint64_t* sample_keys, int64_t per_sample,
+                int64_t t, int64_t n, float alpha_s, float sigma_s, float c_x, float c_0, float c_1, float inv_r0, float c_z,
+                float clip, void* stream) {
+  BG_REQUIRE(eps_cond && x && out && n > 0, "dpm_step: bad arguments");
+  BG_REQUIRE(hist || c_1 == 0.f, "dpm_step: a second-order step (c_1 != 0) needs hist");
+  BG_REQUIRE(!sample_keys || (per_sample > 0 && n % per_sample == 0),
+             "dpm_step: n must be a positive multiple of per_sample");
+  BG_REQUIRE(t >= 0 && t <= 0xFFFFFFFFll, "dpm_step: t must be a 32-bit unsigned value");
+  BG_REQUIRE(alpha_s > 0.f, "dpm_step: alpha_s must be positive");
+  DpmP p = {};
+  p.eps_c = eps_cond; p.eps_u = eps_uncond; p.x = x; p.noise = noise; p.out = out; p.hist = hist; p.n = n; p.w = cfg_w;
+  p.alpha_s = alpha_s; p.sigma_s = sigma_s; p.c_x = c_x; p.c_0 = c_0; p.c_1 = c_1; p.inv_r0 = inv_r0; p.c_z = c_z;
+  p.clip = clip; p.t = t; p.seed = seed; p.offset = offset;
+  return launch_dpm(p, sample_keys, per_sample, stream);
+}
+
+int bg_dpm_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out, float* hist,
+                    uint64_t seed, uint64_t offset0, uint64_t offset_stride, const uint64_t* sample_keys, int64_t per_sample,
+                    const int64_t* t_cur, int64_t n, const float* coef_table, const int32_t* step, float clip, void* stream) {
+  BG_REQUIRE(eps_cond && x && out && hist && n > 0 && coef_table && step, "dpm_step_tab: bad arguments");
+  BG_REQUIRE(!sample_keys || (t_cur && per_sample > 0 && n % per_sample == 0),
+             "dpm_step_tab: keyed noise needs t_cur and n a positive multiple of per_sample");
+  DpmP p = {};
+  p.eps_c = eps_cond; p.eps_u = eps_uncond; p.x = x; p.out = out; p.hist = hist; p.n = n; p.w = cfg_w; p.clip = clip;
+  p.seed = seed; p.offset = offset0; p.offset_stride = offset_stride;
+  p.coef = coef_table; p.step = step; p.t_cur = reinterpret_cast<const long long*>(t_cur);
+  return launch_dpm(p, sample_keys, per_sample, stream);
 }
 
 static int launch_replace(ReplaceP& p, const uint64_t* sample_keys, int64_t per_sample, void* stream) {

@@ -6,8 +6,9 @@ reshapes (sample.py:284-294).  Differences, all result-preserving:
   * no D2H/H2D round trips: dedup runs as device kernels (csrc/dedup.cu), timesteps are device-resident views;
   * CFG combine is fused into the DDPM update kernel (PNDM steps combine with one bg_axpby);
   * three schedules: "reference" = the shipped PNDM(200)[:158] + DDPM(1000)[-250:] hybrid, "ddpm" = N DDPM steps for
-    every stage, which is BASELINE.json's benchmark definition (N = 1000), and "ddim" = N DDIM steps for every stage
-    (few-step sampling of the same DDPM-trained denoisers).
+    every stage, which is BASELINE.json's benchmark definition (N = 1000), "ddim" = N DDIM steps for every stage
+    (few-step sampling of the same DDPM-trained denoisers) and "dpm" = N DPM-Solver++ steps for every stage (the
+    second-order multistep sampler of the same denoisers).
 Everything past sample.py:299 (OpenCASCADE post-processing) is out of scope (SURVEY.md section 2).
 
 Batch sharding across GPUs: samples are independent through every stage, so each rank runs its own shard and there is
@@ -21,7 +22,8 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import torch
 
 from . import _ffi
-from .schedulers import DDIMScheduler, DDPMScheduler, PNDMScheduler, sample_keys, sample_seed
+from .schedulers import (DPM_ALGORITHMS, DDIMScheduler, DDPMScheduler, DPMSolverMultistepScheduler, PNDMScheduler,
+                         sample_keys, sample_seed)
 
 NOISE_MODES = ("batch", "per_sample")
 
@@ -38,10 +40,13 @@ class CascadeConfig:
     class_label: int = 0                 # TEXT2INT[...] when use_cf
     bbox_threshold: float = 0.08         # eval_config.yaml:10
     guidance_w: float = 0.6              # sample.py:49
-    schedule: str = "reference"          # "reference" | "ddpm" | "ddim"
+    schedule: str = "reference"          # "reference" | "ddpm" | "ddim" | "dpm"
     ddpm_steps: int = 1000               # per stage, schedule == "ddpm"
     ddim_steps: int = 50                 # per stage, schedule == "ddim"
     ddim_eta: float = 0.0                # schedule == "ddim": 0 = deterministic DDIM, 1 = DDPM-like noise
+    dpm_steps: int = 20                  # per stage, schedule == "dpm"
+    dpm_order: int = 2                   # schedule == "dpm": 1 (DDIM-like) or 2 (DPM-Solver++ 2M)
+    dpm_algorithm: str = "dpmsolver++"   # schedule == "dpm": "dpmsolver++" (ODE) or "sde-dpmsolver++" (SDE)
     dense_masks: bool = False            # True: skip dedup, every slot valid (the dense-FLOP benchmark mode)
     ragged_masks: bool = False           # benchmark only: synthetic masks shaped like a trained model's output (random-init
                                          # weights never produce duplicates): 1/8..1/2 of the faces valid, 3..E/3 edges each
@@ -136,12 +141,20 @@ def per_sample_seeds(cfg: CascadeConfig) -> Optional[List[int]]:
 
 
 def check_schedule(cfg: CascadeConfig) -> None:
-    """raises ValueError on out-of-range DDIM settings (ddim_steps outside [1, 1000], ddim_eta < 0)"""
+    """raises ValueError on out-of-range DDIM settings (ddim_steps outside [1, 1000], ddim_eta < 0) and DPM settings
+    (dpm_steps outside [1, 1000], dpm_order not 1 or 2, an unknown dpm_algorithm)"""
     if cfg.schedule == "ddim":
         if not 1 <= int(cfg.ddim_steps) <= 1000:
             raise ValueError(f"CascadeConfig.ddim_steps must be in [1, 1000], got {cfg.ddim_steps}")
         if not float(cfg.ddim_eta) >= 0.0:
             raise ValueError(f"CascadeConfig.ddim_eta must be >= 0, got {cfg.ddim_eta}")
+    if cfg.schedule == "dpm":
+        if not 1 <= int(cfg.dpm_steps) <= 1000:
+            raise ValueError(f"CascadeConfig.dpm_steps must be in [1, 1000], got {cfg.dpm_steps}")
+        if cfg.dpm_order not in (1, 2):
+            raise ValueError(f"CascadeConfig.dpm_order must be 1 or 2, got {cfg.dpm_order}")
+        if cfg.dpm_algorithm not in DPM_ALGORITHMS:
+            raise ValueError(f"CascadeConfig.dpm_algorithm must be one of {DPM_ALGORITHMS}, got {cfg.dpm_algorithm!r}")
 
 
 @dataclass
@@ -178,7 +191,7 @@ def check_completion(cfg: CascadeConfig, known: Completion) -> torch.Tensor:
     """raises on a Completion `cfg` cannot run (host checks only; Cascade.run adds the duplicate-face check on the
     device); returns n_faces as a CPU int64 tensor"""
     if cfg.schedule == "reference":
-        raise NotImplementedError("completion needs schedule='ddpm' or 'ddim': PNDM's Runge-Kutta steps advance from a "
+        raise NotImplementedError("completion needs schedule='ddpm', 'ddim' or 'dpm': PNDM's Runge-Kutta steps advance from a "
                                   "sample stored earlier (cur_sample), so known tokens cannot be replaced between them")
     if cfg.dense_masks or cfg.ragged_masks:
         raise ValueError("completion runs the de-duplication; dense_masks and ragged_masks are benchmark modes")
@@ -268,6 +281,13 @@ class Cascade:
         self.ddim = DDIMScheduler(num_train_timesteps=1000, beta_schedule="linear", prediction_type="epsilon",
                                   beta_start=0.0001, beta_end=0.02, clip_sample=True, clip_sample_range=3,
                                   set_alpha_to_one=True)
+        self.dpm = self._dpm_scheduler(2, "dpmsolver++")
+
+    @staticmethod
+    def _dpm_scheduler(order: int, algorithm: str) -> DPMSolverMultistepScheduler:
+        return DPMSolverMultistepScheduler(num_train_timesteps=1000, beta_schedule="linear", prediction_type="epsilon",
+                                           beta_start=0.0001, beta_end=0.02, solver_order=order,
+                                           algorithm_type=algorithm, clip_sample=True, clip_sample_range=3)
 
     # ------------------------------------------------------------------ one DDPM loop as a replayed CUDA graph
     def _use_graph(self, cfg: CascadeConfig, n_steps: int, tokens: int) -> bool:
@@ -278,14 +298,16 @@ class Cascade:
         # a forward is ~105 launches from Python (~1 ms of host time); below ~100 k tokens the GPU finishes sooner than that
         return n_steps >= 32 and tokens <= 100_000
 
-    def _loop_graph(self, cfg: CascadeConfig, sched, timesteps, x, fwd, known=None):
-        """sched: self.ddpm or self.ddim; timesteps: 1-D int64 CPU tensor; x: (B, ...) fp32 on the device; fwd(x_in, t_dev)
+    def _loop_graph(self, cfg: CascadeConfig, sched, timesteps, x, fwd, known=None, tables=None):
+        """sched: self.ddpm, self.ddim or self.dpm; timesteps: 1-D int64 CPU tensor; x: (B, ...) fp32 on the device; fwd(x_in, t_dev)
         -> eps of a (possibly CFG-doubled) batch.  The loop body of sample.py:145-153 -- [step counter / timestep advance] ->
         forward -> fused scheduler step (CFG combine, x0, clip, DDPM posterior mean or DDIM update, Philox noise) -- is
         captured ONCE and replayed len(timesteps) times: no per-step host work.  Nothing step-specific is a kernel argument:
         the timestep comes from a device scalar, the coefficients from a device table indexed by a device counter
-        (bg_step_advance / bg_ddpm_step_tab / bg_ddim_step_tab).  known: {slots: (values, token mask)} of a completion;
-        bg_replace_known_tab then follows the step inside the captured body."""
+        (bg_step_advance / bg_ddpm_step_tab / bg_ddim_step_tab / bg_dpm_step_tab).  known: {slots: (values, token mask)} of
+        a completion; bg_replace_known_tab then follows the step inside the captured body.  tables: (step coefficients,
+        replacement coefficients) of this segment, required for self.dpm, whose rows depend on the whole loop; its history
+        buffer `hist` lives in the scheduler, so it carries over from one segment to the next."""
         dev = self.device
         lib = _ffi.lib()
         T = len(timesteps)
@@ -293,7 +315,12 @@ class Cascade:
         xb = x.detach().float().contiguous().clone()
         n = xb.numel()
         ddim = isinstance(sched, DDIMScheduler)
-        coef = (sched.coefficient_table(timesteps, cfg.ddim_eta) if ddim else sched.coefficient_table(timesteps)).to(dev)
+        dpm = isinstance(sched, DPMSolverMultistepScheduler)
+        if dpm:
+            coef = tables[0].to(dev)
+            hist = sched.history(xb)
+        else:
+            coef = (sched.coefficient_table(timesteps, cfg.ddim_eta) if ddim else sched.coefficient_table(timesteps)).to(dev)
         ts = timesteps.to(device=dev, dtype=torch.int64).contiguous()
         step = torch.full((1,), -1, dtype=torch.int32, device=dev)
         t_cur = torch.zeros(1, dtype=torch.int64, device=dev)
@@ -306,7 +333,7 @@ class Cascade:
         clip = float(sched.config.clip_sample_range) if sched.config.clip_sample else 0.0
         if known is not None:
             kn, km = known[xb.shape[1]]
-            rtab = sched.replace_table(timesteps).to(dev)
+            rtab = (tables[1] if dpm else sched.replace_table(timesteps)).to(dev)
             rseed = 0 if keyed else sched.replace_seed()
 
         def replace(st):
@@ -321,7 +348,12 @@ class Cascade:
             pred = fwd(torch.cat([xb, xb], 0) if cfg.use_cf else xb, t_cur)
             pc = pred[:B] if cfg.use_cf else pred
             pu = pred[B:] if cfg.use_cf else None
-            if ddim:
+            if dpm:
+                _ffi.check(lib.bg_dpm_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(),
+                                               xb.data_ptr(), hist.data_ptr(), seed, off0, stride, _ffi.ptr(keys), n // B,
+                                               t_cur.data_ptr(), n, coef.data_ptr(), step.data_ptr(), clip, st),
+                           "bg_dpm_step_tab")
+            elif ddim:
                 _ffi.check(lib.bg_ddim_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(),
                                                 xb.data_ptr(), seed, off0, stride, _ffi.ptr(keys), n // B, t_cur.data_ptr(),
                                                 n, coef.data_ptr(), step.data_ptr(), clip, 0, st), "bg_ddim_step_tab")
@@ -337,12 +369,15 @@ class Cascade:
 
         # warm-up outside the capture (packs the weights, allocates the workspace), then rewind the state it touched
         x0 = xb.clone()
+        h0 = hist.clone() if dpm else None
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):
             body()
         torch.cuda.current_stream(dev).wait_stream(side)
         xb.copy_(x0)
+        if dpm:
+            hist.copy_(h0)
         step.fill_(-1)
         g = torch.cuda.CUDAGraph()
         l0 = lib.bg_launch_count()
@@ -352,7 +387,9 @@ class Cascade:
         for _ in range(T):
             g.replay()
         _ffi.note_replay(per_replay, T)
-        if not keyed and (not ddim or cfg.ddim_eta > 0):     # DDIM draws (and advances the stream) only when eta > 0
+        # DDIM draws (and advances the stream) only when eta > 0, DPM-Solver++ only in its SDE form
+        draws = cfg.ddim_eta > 0 if ddim else (sched.config.algorithm_type == "sde-dpmsolver++" if dpm else True)
+        if not keyed and draws:
             sched.advance_philox(n, T)
         self.last_graph_steps = getattr(self, "last_graph_steps", 0) + T
         return xb
@@ -365,7 +402,7 @@ class Cascade:
         every step (sched.replace_known); rnoise_fn(k, shape) -> explicit replacement noise (k = -1 before the first step)."""
         B = x.shape[0]
         k = 0
-        fused = isinstance(sched, (DDPMScheduler, DDIMScheduler))    # CFG combine and noise inside the step kernel
+        fused = isinstance(sched, (DDPMScheduler, DDIMScheduler, DPMSolverMultistepScheduler))   # CFG, noise in the kernel
         if known is not None and len(timesteps) > 0:
             x = self._replace(sched, known, x, timesteps[0], -1, rnoise_fn, initial=True)
         if fused and noise_fn is None and rnoise_fn is None and gen is None and len(timesteps) > 0 and \
@@ -382,7 +419,12 @@ class Cascade:
                         hi += 1
                 else:
                     hi = len(ts_list)
-                x = self._loop_graph(cfg, sched, timesteps[lo:hi], x, fwd, known)
+                tabs = None
+                if isinstance(sched, DPMSolverMultistepScheduler):
+                    # a segment after the late increase restarts the solver (first order); rows depend on the whole loop
+                    tabs = (sched.coefficient_table(timesteps, restart=lo if lo else None)[lo:hi],
+                            sched.replace_table(timesteps)[lo:hi])
+                x = self._loop_graph(cfg, sched, timesteps[lo:hi], x, fwd, known, tabs)
                 lo = hi
             return x
         ts_dev = timesteps.to(self.device)
@@ -422,8 +464,12 @@ class Cascade:
         return sched.replace_known(x, kn, km, t, noise=nz, out=None if initial else x, initial=initial)
 
     def _fused_step(self, cfg, sched, k, t, x, pred, gen, noise_fn, **cf):
-        """one DDPM or DDIM step; explicit noise from noise_fn on the steps where diffusers draws it: DDPM at t > 0, DDIM
-        on every step when eta > 0"""
+        """one DDPM, DDIM or DPM-Solver++ step; explicit noise from noise_fn on the steps where diffusers draws it: DDPM at
+        t > 0, DDIM on every step when eta > 0, DPM-Solver++ on every step of its SDE form"""
+        if isinstance(sched, DPMSolverMultistepScheduler):
+            sde = sched.config.algorithm_type == "sde-dpmsolver++"
+            nz = noise_fn(k, x.shape).to(self.device) if (noise_fn is not None and sde) else None
+            return sched.step(pred, t, x, generator=gen, variance_noise=nz, **cf).prev_sample
         if isinstance(sched, DDIMScheduler):
             nz = noise_fn(k, x.shape).to(self.device) if (noise_fn is not None and cfg.ddim_eta > 0) else None
             return sched.step(pred, t, x, eta=cfg.ddim_eta, generator=gen, variance_noise=nz, **cf).prev_sample
@@ -435,7 +481,10 @@ class Cascade:
     def _stage(self, cfg, x, fwd, label2, gen, hybrid_ddpm_tail: bool, on_step=None, noise_fn=None, name="surfPos",
                known=None, rnoise_fn=None):
         seeds = getattr(self, "_sample_seeds", None)
-        noisy = self.ddim if cfg.schedule == "ddim" else self.ddpm
+        if cfg.schedule == "dpm" and (self.dpm.config.solver_order, self.dpm.config.algorithm_type) != \
+                (cfg.dpm_order, cfg.dpm_algorithm):
+            self.dpm = self._dpm_scheduler(cfg.dpm_order, cfg.dpm_algorithm)
+        noisy = {"ddim": self.ddim, "dpm": self.dpm}.get(cfg.schedule, self.ddpm)
         if seeds is not None:
             noisy.set_sample_keys(sample_seeds=seeds, stage=self._STAGE_ID[name])
         else:
@@ -443,6 +492,9 @@ class Cascade:
         if cfg.schedule == "ddim":
             self.ddim.set_timesteps(cfg.ddim_steps)
             return self._loop(cfg, self.ddim, self.ddim.timesteps, x, fwd, label2, gen, on_step, noise_fn, known, rnoise_fn)
+        if cfg.schedule == "dpm":
+            self.dpm.set_timesteps(cfg.dpm_steps)
+            return self._loop(cfg, self.dpm, self.dpm.timesteps, x, fwd, label2, gen, on_step, noise_fn, known, rnoise_fn)
         if cfg.schedule == "ddpm":
             self.ddpm.set_timesteps(cfg.ddpm_steps)
             return self._loop(cfg, self.ddpm, self.ddpm.timesteps, x, fwd, label2, gen, on_step, noise_fn, known, rnoise_fn)
@@ -505,12 +557,13 @@ class Cascade:
     @torch.no_grad()
     def run(self, cfg: CascadeConfig, init_noise: Optional[Dict[str, torch.Tensor]] = None, step_noise=None,
             known: Optional[Completion] = None, replace_noise=None):
-        """step_noise(stage_name, k, shape) -> tensor: explicit DDPM / DDIM step noise of step k (parity runs; DDPM draws it
-        at t > 0, DDIM on every step when ddim_eta > 0); default = in-kernel Philox
+        """step_noise(stage_name, k, shape) -> tensor: explicit DDPM / DDIM / DPM step noise of step k (parity runs; DDPM
+        draws it at t > 0, DDIM on every step when ddim_eta > 0, DPM on every step of "sde-dpmsolver++"); default = in-kernel
+        Philox
         keyed by (cfg.seed, rank, stage): reproducible from cfg.seed, independent across ranks and stages.
         cfg.noise == "per_sample": initial and step noise come from each sample's own streams (bg_randn_keyed and the keyed
         step kernels), so sample b's outputs depend on its seed alone; init_noise / step_noise still take precedence.
-        known: a Completion (schedules "ddpm" and "ddim"): every stage that has known tokens replaces them before its
+        known: a Completion (schedules "ddpm", "ddim" and "dpm"): every stage that has known tokens replaces them before its
         first step and after every step with the known values noised to the step's level, so the rest is generated
         around them; the known parts come out as given, bit for bit.  replace_noise(stage_name, k, shape) -> tensor:
         explicit noise of that replacement (k = -1 before the first step; parity runs), mirroring step_noise."""

@@ -1,5 +1,6 @@
-"""Drop-in DDPMScheduler / PNDMScheduler with the diffusers 0.27 interface used by the reference, and DDIMScheduler
-(diffusers' few-step sampler for the same epsilon-prediction models; not used by the reference).
+"""Drop-in DDPMScheduler / PNDMScheduler with the diffusers 0.27 interface used by the reference, and DDIMScheduler and
+DPMSolverMultistepScheduler (diffusers' few-step samplers for the same epsilon-prediction models; not used by the
+reference).
 
 Call sites mirrored (all in the reference): constructors sample.py:101-117 and trainer.py:285-292;
 `set_timesteps(n)` + `.timesteps[...]` slicing sample.py:128-129,144-145; `.step(pred, t, x).prev_sample`
@@ -7,7 +8,7 @@ sample.py:137,153,202,222,236,282; `.add_noise(x, noise, t)` trainer.py:348; `.c
 
 Host side (this file): the beta / alphas_cumprod tables and the per-step scalar coefficients, computed with the same
 fp32 torch-CPU operations diffusers uses (SURVEY.md Appendix A.3/A.4).  Device side: ONE fused kernel per step
-(bg_ddpm_step / bg_ddim_step / bg_pndm_step in csrc/sched.cu) instead of ~15 scalar-broadcast launches.  No CPU tensor path:
+(bg_ddpm_step / bg_ddim_step / bg_dpm_step / bg_pndm_step in csrc/sched.cu) instead of ~15 scalar-broadcast launches.  No CPU tensor path:
 `step` on a CPU sample raises.
 """
 from __future__ import annotations
@@ -110,7 +111,7 @@ def _generator_noise(x: torch.Tensor, generator) -> torch.Tensor:
 
 
 class _NoiseStreams:
-    """The in-kernel noise sources shared by the fused DDPM and DDIM steps: one batch-wide Philox stream
+    """The in-kernel noise sources shared by the fused DDPM, DDIM and DPM-Solver++ steps: one batch-wide Philox stream
     (set_noise_seed) or per-sample streams (set_sample_keys)."""
 
     def _init_noise_streams(self):
@@ -444,6 +445,244 @@ class DDIMScheduler(_NoiseStreams):
                                               n // x.shape[0], t, n, sb, sa, sa_prev, c_dir, sigma,
                                               float(self.config.clip_sample_range) if self.config.clip_sample else 0.0,
                                               int(bool(use_clipped_model_output)), _ffi.current_stream()), "bg_ddim_step")
+        return SchedulerOutput(dst) if return_dict else (dst,)
+
+    def add_noise(self, original_samples, noise, timesteps):
+        return DDPMScheduler.add_noise(self, original_samples, noise, timesteps)
+
+    def __len__(self):
+        return self.config.num_train_timesteps
+
+
+DPM_ALGORITHMS = ("dpmsolver++", "sde-dpmsolver++")
+
+
+def dpm_timesteps(num_train_timesteps: int, num_inference_steps: int, spacing: str, steps_offset: int = 0) -> np.ndarray:
+    """int64 timesteps of diffusers' DPMSolverMultistepScheduler.set_timesteps (lambda_min_clipped = -inf)"""
+    n, last = num_inference_steps, num_train_timesteps
+    if spacing == "linspace":
+        return np.linspace(0, last - 1, n + 1).round()[::-1][:-1].copy().astype(np.int64)
+    if spacing == "leading":
+        ratio = last // (n + 1)
+        return (np.arange(0, n + 1) * ratio).round()[::-1][:-1].copy().astype(np.int64) + steps_offset
+    if spacing == "trailing":
+        return np.arange(last, 0, -num_train_timesteps / n).round().copy().astype(np.int64) - 1
+    raise NotImplementedError(f"timestep_spacing={spacing!r}")
+
+
+class DPMSolverMultistepScheduler(_NoiseStreams):
+    """diffusers 0.27 DPMSolverMultistepScheduler for epsilon-prediction models: the DPM-Solver++ multistep ("2M") sampler,
+    deterministic ("dpmsolver++") or stochastic ("sde-dpmsolver++"), of a model trained as a DDPM.  One fused kernel per
+    step (bg_dpm_step); the per-step scalars are computed here in fp32 torch as diffusers computes them.  The history of
+    data predictions (diffusers' model_outputs list) is one device tensor of the sample's shape, `hist`, that the kernel
+    reads and overwrites in place.
+
+    Extras over diffusers: `clip_sample` / `clip_sample_range` clamp the data prediction x0 before it is used and stored
+    (static thresholding; off by default, as in diffusers, which has no such option).  A `step` on a sample whose shape
+    differs from the history's restarts the solver: that step is first order and the history is reallocated."""
+
+    def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.0001, beta_end: float = 0.02,
+                 beta_schedule: str = "linear", trained_betas=None, solver_order: int = 2,
+                 prediction_type: str = "epsilon", thresholding: bool = False, dynamic_thresholding_ratio: float = 0.995,
+                 sample_max_value: float = 1.0, algorithm_type: str = "dpmsolver++", solver_type: str = "midpoint",
+                 lower_order_final: bool = True, euler_at_final: bool = False, use_karras_sigmas: bool = False,
+                 use_lu_lambdas: bool = False, final_sigmas_type: str = "zero", lambda_min_clipped: float = -float("inf"),
+                 variance_type=None, timestep_spacing: str = "linspace", steps_offset: int = 0,
+                 clip_sample: bool = False, clip_sample_range: float = 1.0, **unused):
+        if prediction_type != "epsilon" or thresholding or use_karras_sigmas or use_lu_lambdas or \
+                solver_order not in (1, 2) or algorithm_type not in DPM_ALGORITHMS or solver_type != "midpoint" or \
+                final_sigmas_type != "zero" or lambda_min_clipped != -float("inf") or trained_betas is not None or \
+                variance_type is not None or timestep_spacing not in ("linspace", "leading", "trailing"):
+            raise NotImplementedError("only prediction_type='epsilon', solver_order 1 or 2, algorithm_type 'dpmsolver++' or "
+                                      "'sde-dpmsolver++', solver_type='midpoint', final_sigmas_type='zero', "
+                                      "timestep_spacing 'linspace' / 'leading' / 'trailing'; no thresholding, Karras or Lu "
+                                      "sigmas, lambda_min_clipped, variance_type or trained_betas")
+        self.config = SimpleNamespace(num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
+                                      beta_schedule=beta_schedule, trained_betas=trained_betas, solver_order=solver_order,
+                                      prediction_type=prediction_type, thresholding=thresholding,
+                                      dynamic_thresholding_ratio=dynamic_thresholding_ratio,
+                                      sample_max_value=sample_max_value, algorithm_type=algorithm_type,
+                                      solver_type=solver_type, lower_order_final=lower_order_final,
+                                      euler_at_final=euler_at_final, use_karras_sigmas=use_karras_sigmas,
+                                      use_lu_lambdas=use_lu_lambdas, final_sigmas_type=final_sigmas_type,
+                                      lambda_min_clipped=lambda_min_clipped, variance_type=variance_type,
+                                      timestep_spacing=timestep_spacing, steps_offset=steps_offset,
+                                      clip_sample=clip_sample, clip_sample_range=clip_sample_range)
+        self.betas = _betas(num_train_timesteps, beta_start, beta_end, beta_schedule)
+        self.alphas = 1.0 - self.betas
+        self.alphas_cumprod = torch.cumprod(self.alphas, dim=0)
+        self.alpha_t = torch.sqrt(self.alphas_cumprod)
+        self.sigma_t = torch.sqrt(1 - self.alphas_cumprod)
+        self.lambda_t = torch.log(self.alpha_t) - torch.log(self.sigma_t)
+        self.sigmas = ((1 - self.alphas_cumprod) / self.alphas_cumprod) ** 0.5
+        self.init_noise_sigma = 1.0
+        self.num_inference_steps = None
+        self.timesteps = torch.from_numpy(np.linspace(0, num_train_timesteps - 1, num_train_timesteps,
+                                                      dtype=np.float32)[::-1].copy())
+        self.lower_order_nums = 0
+        self._step_index = None
+        self.hist = None
+        self._init_noise_streams()
+
+    @property
+    def model_outputs(self):
+        """diffusers' history list: the last data prediction (the device tensor `hist`) at the end once a step has run"""
+        last = [self.hist] if self.lower_order_nums >= 1 else [None]
+        return [None] * (self.config.solver_order - 1) + last
+
+    @property
+    def step_index(self):
+        return self._step_index
+
+    def set_timesteps(self, num_inference_steps: int, device=None):
+        n_train = self.config.num_train_timesteps
+        if num_inference_steps > n_train:
+            raise ValueError("num_inference_steps cannot exceed num_train_timesteps")
+        ts = dpm_timesteps(n_train, num_inference_steps, self.config.timestep_spacing, self.config.steps_offset)
+        sig = (((1 - self.alphas_cumprod) / self.alphas_cumprod) ** 0.5).numpy()
+        sig = np.interp(ts, np.arange(0, len(sig)), sig)
+        self.sigmas = torch.from_numpy(np.concatenate([sig, [0]]).astype(np.float32))
+        self.timesteps = torch.from_numpy(ts).to(dtype=torch.int64)
+        self.num_inference_steps = len(ts)
+        self.lower_order_nums = 0
+        self._step_index = None
+
+    def scale_model_input(self, sample, timestep=None):
+        return sample
+
+    def index_for_timestep(self, timestep) -> int:
+        """diffusers' rule: the position of `timestep` in the table, its second occurrence if it repeats, the last step if
+        it is absent"""
+        cand = (self.timesteps == _as_int(timestep)).nonzero().flatten().tolist()
+        if not cand:
+            return len(self.timesteps) - 1
+        return cand[1] if len(cand) > 1 else cand[0]
+
+    def _alpha_sigma(self, k: int):
+        """(alpha, sigma_t, lambda) of sigmas[k] as fp32 torch scalars (diffusers' _sigma_to_alpha_sigma_t)"""
+        s = self.sigmas[k]
+        alpha = 1 / ((s ** 2 + 1) ** 0.5)
+        sigma = s * alpha
+        return alpha, sigma, torch.log(alpha) - torch.log(sigma)
+
+    def step_order(self, k: int, restart: Optional[int] = None) -> int:
+        """the order of step k of a loop that (re)starts with an empty history at step `restart` (default: the first
+        step): 1 at the restart, at the last step (final sigma = 0) and for solver_order = 1; else 2"""
+        if self.num_inference_steps is None:
+            raise ValueError("Number of inference steps is 'None', you need to run 'set_timesteps' after creating the "
+                             "scheduler")
+        last = k == self.num_inference_steps - 1
+        return 1 if (self.config.solver_order == 1 or k == 0 or k == restart or last) else 2
+
+    def step_coefficients(self, k: int, order: int):
+        """(alpha_s, sigma_s, c_x, c_0, c_1, inv_r0, c_z) of step index k as Python floats (fp32 arithmetic like diffusers'
+        dpm_solver_first_order_update / multistep_dpm_solver_second_order_update)"""
+        alpha_t, sigma_t, lambda_t = self._alpha_sigma(k + 1)
+        alpha_s, sigma_s, lambda_s = self._alpha_sigma(k)
+        h = lambda_t - lambda_s
+        if self.config.algorithm_type == "dpmsolver++":
+            c_x, c_0, c_z = sigma_t / sigma_s, -(alpha_t * (torch.exp(-h) - 1.0)), 0.0
+            c_1 = -(0.5 * (alpha_t * (torch.exp(-h) - 1.0)))
+        else:
+            c_x, c_0 = sigma_t / sigma_s * torch.exp(-h), alpha_t * (1 - torch.exp(-2.0 * h))
+            c_1 = 0.5 * (alpha_t * (1 - torch.exp(-2.0 * h)))
+            c_z = sigma_t * torch.sqrt(1.0 - torch.exp(-2.0 * h))
+        inv_r0 = 0.0
+        if order == 2:
+            lambda_s1 = self._alpha_sigma(k - 1)[2]
+            inv_r0 = float(1.0 / ((lambda_s - lambda_s1) / h))
+        else:
+            c_1 = 0.0
+        return float(alpha_s), float(sigma_s), float(c_x), float(c_0), float(c_1), inv_r0, float(c_z)
+
+    def coefficient_table(self, timesteps=None, restart: Optional[int] = None) -> torch.Tensor:
+        """[len(timesteps), 7] fp32 (CPU): step_coefficients of every step of a denoising loop over `timesteps` (default
+        the whole table; a consecutive run of it), the order from step_order(k, restart) with `restart` a row of this
+        table -- the device table that bg_dpm_step_tab indexes with its step counter when the loop is captured in a CUDA
+        graph.  The rows depend on the neighbouring sigmas and the global step index, so a loop split into graph segments
+        slices the table of the whole loop."""
+        k0 = 0 if timesteps is None or len(timesteps) == 0 else self.index_for_timestep(timesteps[0])
+        T = self.num_inference_steps if timesteps is None else len(timesteps)
+        rows = [self.step_coefficients(k0 + j, self.step_order(k0 + j, None if restart is None else k0 + restart))
+                for j in range(T)]
+        return torch.tensor(rows, dtype=torch.float32).reshape(-1, 7)
+
+    def history(self, x: torch.Tensor) -> torch.Tensor:
+        """the history buffer for samples shaped like x: `hist`, reallocated (zeroed) when x's shape or device differs"""
+        if self.hist is None or tuple(self.hist.shape) != tuple(x.shape) or self.hist.device != x.device:
+            self.hist = torch.zeros(x.shape, dtype=torch.float32, device=x.device)
+        return self.hist
+
+    def _abar_after(self, k: int) -> torch.Tensor:
+        s = self.sigmas[k + 1]
+        return 1.0 / (1.0 + s * s)
+
+    def _abar_prev(self, t: int) -> torch.Tensor:
+        """abar of the level step(t) leaves x at: 1 / (1 + sigma_next^2), exactly 1 after the last step (sigma = 0).  The
+        step just taken when it was at t (timesteps may repeat), else diffusers' index rule."""
+        if self.num_inference_steps is None:
+            raise ValueError("Number of inference steps is 'None', you need to run 'set_timesteps' after creating the "
+                             "scheduler")
+        k = self._step_index - 1 if self._step_index and int(self.timesteps[self._step_index - 1]) == int(t) else \
+            self.index_for_timestep(t)
+        return self._abar_after(k)
+
+    def replace_table(self, timesteps) -> torch.Tensor:
+        """[len(timesteps), 2] fp32 (CPU): replace_coefficients of every step of a loop over a consecutive run of the
+        timestep table, row by row (repeated timesteps keep their own rows)"""
+        k0 = self.index_for_timestep(timesteps[0]) if len(timesteps) else 0
+        rows = []
+        for j in range(len(timesteps)):
+            a = self._abar_after(k0 + j)
+            rows.append((float(a ** 0.5), float((1 - a) ** 0.5)))
+        return torch.tensor(rows, dtype=torch.float32).reshape(-1, 2)
+
+    def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, generator=None,
+             variance_noise: Optional[torch.Tensor] = None, return_dict: bool = True,
+             model_output_uncond: Optional[torch.Tensor] = None, guidance_w: float = 0.0,
+             out: Optional[torch.Tensor] = None):
+        """x at the next timestep of diffusers' DPM-Solver++ step.  In SDE mode the noise comes from `variance_noise`, else
+        `generator` (one, or a list with one per batch element), else the in-kernel stream (per sample after
+        set_sample_keys, else batch-wide), and is drawn on every step, the last one included, as diffusers draws it.
+        Extras over diffusers, as in DDIMScheduler.step: `model_output_uncond` + `guidance_w` fuse the classifier-free
+        combine, `out` is the destination (may be `sample`).  pred_original_sample is not returned (None)."""
+        if self.num_inference_steps is None:
+            raise ValueError("Number of inference steps is 'None', you need to run 'set_timesteps' after creating the "
+                             "scheduler")
+        sde = self.config.algorithm_type == "sde-dpmsolver++"
+        x, eps, eps_u, dst = _step_tensors("DPMSolverMultistepScheduler.step", model_output, sample, model_output_uncond,
+                                           variance_noise if sde else None, out)
+        if self._step_index is None:
+            self._step_index = self.index_for_timestep(timestep)
+        k = self._step_index
+        if self.hist is None or tuple(self.hist.shape) != tuple(x.shape) or self.hist.device != x.device:
+            self.lower_order_nums = 0           # a new shape restarts the solver: its history is of another sample
+        hist = self.history(x)
+        last = k == len(self.timesteps) - 1
+        order = 1 if (self.config.solver_order == 1 or self.lower_order_nums < 1 or last) else 2
+        coefs = self.step_coefficients(k, order)
+        t = _as_int(timestep)
+        noise, seed, offset, keys = None, 0, 0, None
+        n = x.numel()
+        if sde:
+            noise = variance_noise if variance_noise is not None else \
+                (_generator_noise(x, generator) if generator is not None else None)
+            if noise is not None:
+                noise = noise.to(device=x.device, dtype=torch.float32).contiguous()
+            elif self._sample_seeds is not None:
+                keys = self.sample_key_tensor(x.shape[0], x.device)
+            else:
+                seed, offset, _ = self.philox_stream(n)
+                self.advance_philox(n, 1)
+        clip = float(self.config.clip_sample_range) if self.config.clip_sample else 0.0
+        with torch.cuda.device(x.device):
+            _ffi.check(_ffi.lib().bg_dpm_step(eps.data_ptr(), _ffi.ptr(eps_u), float(guidance_w), x.data_ptr(),
+                                             dst.data_ptr(), hist.data_ptr(), _ffi.ptr(noise), seed, offset,
+                                             _ffi.ptr(keys), n // x.shape[0], t, n, *coefs, clip, _ffi.current_stream()),
+                       "bg_dpm_step")
+        if self.lower_order_nums < self.config.solver_order:
+            self.lower_order_nums += 1
+        self._step_index += 1
         return SchedulerOutput(dst) if return_dict else (dst,)
 
     def add_noise(self, original_samples, noise, timesteps):

@@ -196,6 +196,30 @@ int bg_ddim_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w
                      uint64_t offset0, uint64_t offset_stride, const uint64_t* sample_keys, int64_t per_sample,
                      const int64_t* t_cur, int64_t n, const float* coef_table, const int32_t* step, float clip,
                      int32_t use_clipped_eps, void* stream);
+/* DPM-Solver++ multistep step (diffusers DPMSolverMultistepScheduler, prediction_type "epsilon", solver_type "midpoint",
+ * algorithm_type "dpmsolver++" or "sde-dpmsolver++"), fp32 with every operation rounded in diffusers' order:
+ * eps = eps_cond if eps_uncond == NULL else eps_cond*(1+w) - eps_uncond*w            (CFG, as bg_ddpm_step)
+ * x0  = clamp((x - sigma_s*eps) / alpha_s, -clip, clip)   (clip <= 0: no clamp; the data prediction)
+ * D1  = (x0 - hist) * inv_r0;   hist = x0                  (hist holds the previous step's x0; updated in place)
+ * out = c_x*x + c_0*x0 + c_1*D1 + c_z*noise
+ * With h = lambda_t - lambda_s (lambda = log alpha - log sigma): ODE c_x = sigma_t/sigma_s, c_0 = -alpha_t(e^-h - 1),
+ * c_1 = c_0/2 (second order) or 0 (first order), c_z = 0; SDE c_x = sigma_t/sigma_s e^-h, c_0 = alpha_t(1 - e^-2h),
+ * c_1 = c_0/2 or 0, c_z = sigma_t sqrt(1 - e^-2h).  Computed by the host scheduler.  c_1 == 0 never reads hist, and
+ * hist == NULL (allowed only then) skips the store.  out may alias x; hist must alias neither.  noise (only read when
+ * c_z != 0): as bg_ddim_step (explicit tensor, else the per-sample streams at domain 0 and timestep t, else the batch
+ * stream (seed, offset)).  BG_STATUS_BAD_ARG, launching nothing: NULL pointers, hist == NULL with c_1 != 0,
+ * alpha_s <= 0, t outside 32 bits, keyed with per_sample <= 0 or n not a multiple of per_sample. */
+int bg_dpm_step(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out, float* hist,
+                const float* noise, uint64_t seed, uint64_t offset, const uint64_t* sample_keys, int64_t per_sample,
+                int64_t t, int64_t n, float alpha_s, float sigma_s, float c_x, float c_0, float c_1, float inv_r0, float c_z,
+                float clip, void* stream);
+/* table-driven form for graph capture: coef_table[k][7] = (alpha_s, sigma_s, c_x, c_0, c_1, inv_r0, c_z) of step
+ * k = *step (bg_step_advance), batch-stream counter offset0 + k * offset_stride, or, when sample_keys != NULL, the
+ * per-sample streams at the timestep *t_cur (t_cur may be NULL only without keys).  hist must not be NULL.
+ * Bit-identical to bg_dpm_step with the same coefficients and noise. */
+int bg_dpm_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out, float* hist,
+                    uint64_t seed, uint64_t offset0, uint64_t offset_stride, const uint64_t* sample_keys, int64_t per_sample,
+                    const int64_t* t_cur, int64_t n, const float* coef_table, const int32_t* step, float clip, void* stream);
 /* Known-token replacement (B-rep completion; runs after the step kernel, in place on x).  x is n fp32 elements in tokens
  * of per_token consecutive elements; token_mask holds one byte per token (n / per_token).  For every element of a token
  * whose byte is non-zero:  x[i] = sqrt_abar*known[i] + sqrt_one_minus_abar*z  (fmaf(sa, known, sb*z); sa*known when

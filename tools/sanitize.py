@@ -42,6 +42,10 @@ import test_gpu_ddim as DD   # noqa: E402
 run("ddim step", DD.test_step_matches_float64, 0, 10, False, 0.5)
 run("ddim forms", DD.test_eager_keyed_and_table_forms_agree, 7, 0.6, 1)
 run("ddim bad args", DD.test_bad_arguments_are_rejected_and_launch_nothing)
+import test_gpu_dpm as DP   # noqa: E402
+run("dpm step", DP.test_step_matches_float64, 10, "sde-dpmsolver++")
+run("dpm forms", DP.test_eager_keyed_and_table_forms_agree, 7, 0.6)
+run("dpm bad args", DP.test_bad_arguments_are_rejected_and_launch_nothing)
 import test_gpu_completion as CO   # noqa: E402
 run("replace known", CO.test_kernel_matches_float64, 18, 13, "random")
 run("replace forms", CO.test_noise_forms_agree, 6, 7)
