@@ -389,6 +389,134 @@ __global__ void __launch_bounds__(256) replace_known_kernel(const ReplaceP p) {
   }
 }
 
+// RePaint step (diffusers 0.27 RePaintScheduler.step, epsilon prediction): the DDIM update of ddim_step_kernel for the
+// unknown tokens, written with exactly its expressions (so with nothing known and the same noise it is bg_ddim_step bit
+// for bit), and for the elements of tokens whose mask byte is set the known part sa_prev*known + sb_prev*z, written as
+// replace_known_kernel writes it.  One z serves both: the variance term sigma*z and the known part draw the same normal.
+// z is drawn only when sigma != 0 or the group holds a known token: explicit `noise`, else per-sample keys
+// (keyed_normal4, domain 3, counter word k = the entry's index in the stage's RePaint list), else the batch key `seed`
+// over the whole tensor as one sample.  Table form (coef != NULL): (sb, sa, sa_prev, c_dir, sigma, sb_prev) from
+// coef[6 * *step] and k = *step.
+struct RepaintP {
+  const float *eps_c, *eps_u, *x, *noise, *known;
+  float* out;
+  const unsigned char* mask;
+  long long n, per_token, per_sample;
+  float w, sb, sa, sa_prev, c_dir, sigma, sb_prev, clip;
+  unsigned long long seed;
+  const unsigned long long* keys;
+  long long k;
+  const float* coef;
+  const int* step;
+};
+__global__ void __launch_bounds__(256) repaint_step_kernel(const RepaintP p) {
+  float sb = p.sb, sa = p.sa, sa_prev = p.sa_prev, c_dir = p.c_dir, sigma = p.sigma, sb_prev = p.sb_prev;
+  long long k = p.k;
+  if (p.coef) {
+    k = *p.step;
+    const float* cf = p.coef + 6 * k;
+    sb = cf[0]; sa = cf[1]; sa_prev = cf[2]; c_dir = cf[3]; sigma = cf[4]; sb_prev = cf[5];
+  }
+  const long long gps = (p.per_sample + 3) / 4, ng = (p.n / p.per_sample) * gps;
+  for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += (long long)gridDim.x * blockDim.x) {
+    const long long b = g / gps, q = g - b * gps;
+    const long long base = b * p.per_sample, js0 = q * 4;
+    const int cnt = (int)min(4ll, p.per_sample - js0);
+    bool known[4] = {false, false, false, false};
+    bool any = false;
+    if (p.mask) {   // tokens of the group's elements, as replace_known_kernel: one division per group
+      long long tok = (base + js0) / p.per_token, r = base + js0 - tok * p.per_token;
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (j < cnt) {
+          known[j] = p.mask[tok] != 0;
+          any |= known[j];
+          if (++r == p.per_token) { ++tok; r = 0; }
+        }
+    }
+    float z[4] = {0.f, 0.f, 0.f, 0.f};
+    if ((sigma != 0.f || any) && p.noise == nullptr)
+      keyed_normal4(p.keys ? p.keys[b] : p.seed, (unsigned long long)q, (uint32_t)k, 3u, z);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if (j >= cnt) break;
+      const long long i = base + js0 + j;
+      const float zj = p.noise && (sigma != 0.f || known[j]) ? p.noise[i] : z[j];
+      float o;
+      if (known[j]) {
+        const float kv = p.known[i];
+        // sb_prev == 0 (the last step, abar_prev = 1): sa_prev*kv keeps the sign of a zero, so the token ends at known
+        o = sb_prev == 0.f ? __fmul_rn(sa_prev, kv) : __fmaf_rn(sa_prev, kv, __fmul_rn(sb_prev, zj));
+      } else {
+        // the roundings ddim_step_kernel compiles to (its FMA contractions spelled out, so no other contraction can
+        // differ):  e*(1+w) - eu*w;  (x - sb*e) / sa;  sa_prev*x0 + c_dir*e;  + sigma*z
+        float e = p.eps_c[i];
+        if (p.eps_u) e = __fmaf_rn(e, 1.f + p.w, -__fmul_rn(p.eps_u[i], p.w));
+        const float xv = p.x[i];
+        float x0 = __fdiv_rn(__fmaf_rn(-sb, e, xv), sa);
+        if (p.clip > 0.f) x0 = fminf(fmaxf(x0, -p.clip), p.clip);
+        o = __fmaf_rn(sa_prev, x0, __fmul_rn(c_dir, e));
+        if (sigma != 0.f) o = __fmaf_rn(sigma, zj, o);
+      }
+      p.out[i] = o;
+    }
+  }
+}
+
+// RePaint undo (diffusers 0.27 RePaintScheduler.undo_step): n_trans forward-diffusion transitions of one undo entry in
+// registers, in place, x = sqrt(1-beta_i)*x + sqrt(beta_i)*z_i for i = 0..n_trans-1, every product and the sum rounded
+// on their own (the fp32 torch chain).  cf[2i], cf[2i+1] = (sqrt(1-beta), sqrt(beta)) of transition i.  z_i: explicit
+// `noise` of shape (n_trans, n), else per-sample keys (keyed_normal4, domain 4, counter word k * n_trans + i), else the
+// batch key `seed` over the whole tensor as one sample.  Table form (coef != NULL): cf = coef + 2 * n_trans * *step and
+// k = *step.
+struct UndoP {
+  float* x;
+  const float* noise;
+  long long n, per_sample;
+  int n_trans;
+  const float* cf;
+  unsigned long long seed;
+  const unsigned long long* keys;
+  long long k;
+  const float* coef;
+  const int* step;
+};
+__global__ void __launch_bounds__(256) repaint_undo_kernel(const UndoP p) {
+  const float* cf = p.cf;
+  long long k = p.k;
+  if (p.coef) {
+    k = *p.step;
+    cf = p.coef + 2ll * p.n_trans * k;
+  }
+  const long long gps = (p.per_sample + 3) / 4, ng = (p.n / p.per_sample) * gps;
+  for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += (long long)gridDim.x * blockDim.x) {
+    const long long b = g / gps, q = g - b * gps;
+    const long long i0 = b * p.per_sample + q * 4;
+    const int cnt = (int)min(4ll, p.per_sample - q * 4);
+    const unsigned long long key = p.keys ? p.keys[b] : p.seed;
+    float v[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) v[j] = j < cnt ? p.x[i0 + j] : 0.f;
+#pragma unroll 1
+    for (int s = 0; s < p.n_trans; ++s) {
+      const float a = cf[2 * s], c = cf[2 * s + 1];
+      float z[4];
+      if (p.noise) {
+        const float* nz = p.noise + (long long)s * p.n + i0;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) z[j] = j < cnt ? nz[j] : 0.f;
+      } else {
+        keyed_normal4(key, (unsigned long long)q, (uint32_t)(k * p.n_trans + s), 4u, z);
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) v[j] = __fadd_rn(__fmul_rn(a, v[j]), __fmul_rn(c, z[j]));
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      if (j < cnt) p.x[i0 + j] = v[j];
+  }
+}
+
 // one thread: k = ++(*step);  *t_cur = ts[k]   (the denoiser reads its timestep from t_cur, the step kernel reads k)
 __global__ void step_advance_kernel(const long long* __restrict__ ts, int n, int* __restrict__ step, long long* __restrict__ t_cur) {
   int k = *step + 1;
@@ -612,6 +740,81 @@ int bg_replace_known_tab(float* x, const float* known, const uint8_t* token_mask
   p.x = x; p.known = known; p.mask = token_mask; p.n = n; p.per_token = per_token; p.seed = seed;
   p.coef = coef_table; p.step = step; p.t_cur = reinterpret_cast<const long long*>(t_cur);
   return launch_replace(p, sample_keys, per_sample, stream);
+}
+
+static int launch_repaint(RepaintP& p, const uint64_t* sample_keys, int64_t per_sample, void* stream) {
+  p.keys = reinterpret_cast<const unsigned long long*>(sample_keys);
+  p.per_sample = sample_keys ? per_sample : p.n;
+  repaint_step_kernel<<<grid_for((p.n / p.per_sample) * ((p.per_sample + 3) / 4)), 256, 0,
+                        reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch("repaint_step_kernel launch");
+}
+
+int bg_repaint_step(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
+                    const float* known, const uint8_t* token_mask, int64_t per_token, const float* noise, uint64_t seed,
+                    const uint64_t* sample_keys, int64_t per_sample, int64_t k, int64_t n, float sqrt_one_minus_abar,
+                    float sqrt_abar, float sqrt_abar_prev, float c_dir, float sigma, float sqrt_one_minus_abar_prev,
+                    float clip, void* stream) {
+  BG_REQUIRE(eps_cond && x && out && n > 0, "repaint_step: bad arguments");
+  BG_REQUIRE((known == nullptr) == (token_mask == nullptr), "repaint_step: give known and token_mask together or neither");
+  BG_REQUIRE(!token_mask || (per_token > 0 && n % per_token == 0),
+             "repaint_step: n must be a positive multiple of per_token");
+  BG_REQUIRE(!sample_keys || (per_sample > 0 && n % per_sample == 0 && (!token_mask || per_sample % per_token == 0)),
+             "repaint_step: per_sample must be a positive multiple of per_token that divides n");
+  BG_REQUIRE(k >= 0 && k <= 0xFFFFFFFFll, "repaint_step: k must be a 32-bit unsigned value");
+  BG_REQUIRE(sqrt_abar > 0.f, "repaint_step: sqrt_abar must be positive");
+  RepaintP p = {};
+  p.eps_c = eps_cond; p.eps_u = eps_uncond; p.x = x; p.out = out; p.known = known; p.mask = token_mask; p.noise = noise;
+  p.n = n; p.per_token = per_token; p.w = cfg_w; p.sb = sqrt_one_minus_abar; p.sa = sqrt_abar; p.sa_prev = sqrt_abar_prev;
+  p.c_dir = c_dir; p.sigma = sigma; p.sb_prev = sqrt_one_minus_abar_prev; p.clip = clip; p.seed = seed; p.k = k;
+  return launch_repaint(p, sample_keys, per_sample, stream);
+}
+
+int bg_repaint_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
+                        const float* known, const uint8_t* token_mask, int64_t per_token, uint64_t seed,
+                        const uint64_t* sample_keys, int64_t per_sample, int64_t n, const float* coef_table,
+                        const int32_t* step, float clip, void* stream) {
+  BG_REQUIRE(eps_cond && x && out && n > 0 && coef_table && step, "repaint_step_tab: bad arguments");
+  BG_REQUIRE((known == nullptr) == (token_mask == nullptr),
+             "repaint_step_tab: give known and token_mask together or neither");
+  BG_REQUIRE(!token_mask || (per_token > 0 && n % per_token == 0),
+             "repaint_step_tab: n must be a positive multiple of per_token");
+  BG_REQUIRE(!sample_keys || (per_sample > 0 && n % per_sample == 0 && (!token_mask || per_sample % per_token == 0)),
+             "repaint_step_tab: per_sample must be a positive multiple of per_token that divides n");
+  RepaintP p = {};
+  p.eps_c = eps_cond; p.eps_u = eps_uncond; p.x = x; p.out = out; p.known = known; p.mask = token_mask; p.n = n;
+  p.per_token = per_token; p.w = cfg_w; p.clip = clip; p.seed = seed; p.coef = coef_table; p.step = step;
+  return launch_repaint(p, sample_keys, per_sample, stream);
+}
+
+static int launch_undo(UndoP& p, const uint64_t* sample_keys, int64_t per_sample, void* stream) {
+  p.keys = reinterpret_cast<const unsigned long long*>(sample_keys);
+  p.per_sample = sample_keys ? per_sample : p.n;
+  repaint_undo_kernel<<<grid_for((p.n / p.per_sample) * ((p.per_sample + 3) / 4)), 256, 0,
+                        reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch("repaint_undo_kernel launch");
+}
+
+int bg_repaint_undo(float* x, int64_t n, int32_t n_trans, const float* coef, const float* noise, uint64_t seed,
+                    const uint64_t* sample_keys, int64_t per_sample, int64_t k, void* stream) {
+  BG_REQUIRE(x && coef && n > 0 && n_trans > 0, "repaint_undo: bad arguments");
+  BG_REQUIRE(!sample_keys || (per_sample > 0 && n % per_sample == 0),
+             "repaint_undo: n must be a positive multiple of per_sample");
+  BG_REQUIRE(k >= 0 && (k + 1) * (int64_t)n_trans <= 0x100000000ll,
+             "repaint_undo: the counter words k * n_trans + i must be 32-bit unsigned values");
+  UndoP p = {};
+  p.x = x; p.noise = noise; p.n = n; p.n_trans = n_trans; p.cf = coef; p.seed = seed; p.k = k;
+  return launch_undo(p, sample_keys, per_sample, stream);
+}
+
+int bg_repaint_undo_tab(float* x, int64_t n, int32_t n_trans, uint64_t seed, const uint64_t* sample_keys,
+                        int64_t per_sample, const float* coef_table, const int32_t* step, void* stream) {
+  BG_REQUIRE(x && coef_table && step && n > 0 && n_trans > 0, "repaint_undo_tab: bad arguments");
+  BG_REQUIRE(!sample_keys || (per_sample > 0 && n % per_sample == 0),
+             "repaint_undo_tab: n must be a positive multiple of per_sample");
+  UndoP p = {};
+  p.x = x; p.n = n; p.n_trans = n_trans; p.seed = seed; p.coef = coef_table; p.step = step;
+  return launch_undo(p, sample_keys, per_sample, stream);
 }
 
 int bg_step_advance(const int64_t* timesteps, int n_steps, int32_t* step, int64_t* t_cur, void* stream) {

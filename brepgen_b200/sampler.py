@@ -7,8 +7,9 @@ reshapes (sample.py:284-294).  Differences, all result-preserving:
   * CFG combine is fused into the DDPM update kernel (PNDM steps combine with one bg_axpby);
   * three schedules: "reference" = the shipped PNDM(200)[:158] + DDPM(1000)[-250:] hybrid, "ddpm" = N DDPM steps for
     every stage, which is BASELINE.json's benchmark definition (N = 1000), "ddim" = N DDIM steps for every stage
-    (few-step sampling of the same DDPM-trained denoisers) and "dpm" = N DPM-Solver++ steps for every stage (the
-    second-order multistep sampler of the same denoisers).
+    (few-step sampling of the same DDPM-trained denoisers), "dpm" = N DPM-Solver++ steps for every stage (the
+    second-order multistep sampler of the same denoisers) and "repaint" = diffusers' RePaint list of DDIM-form steps and
+    undo steps per stage (resampling, for completion).
 Everything past sample.py:299 (OpenCASCADE post-processing) is out of scope (SURVEY.md section 2).
 
 Batch sharding across GPUs: samples are independent through every stage, so each rank runs its own shard and there is
@@ -23,7 +24,7 @@ import torch
 
 from . import _ffi
 from .schedulers import (DPM_ALGORITHMS, DDIMScheduler, DDPMScheduler, DPMSolverMultistepScheduler, PNDMScheduler,
-                         sample_keys, sample_seed)
+                         RePaintScheduler, repaint_entries, sample_keys, sample_seed)
 
 NOISE_MODES = ("batch", "per_sample")
 
@@ -40,13 +41,17 @@ class CascadeConfig:
     class_label: int = 0                 # TEXT2INT[...] when use_cf
     bbox_threshold: float = 0.08         # eval_config.yaml:10
     guidance_w: float = 0.6              # sample.py:49
-    schedule: str = "reference"          # "reference" | "ddpm" | "ddim" | "dpm"
+    schedule: str = "reference"          # "reference" | "ddpm" | "ddim" | "dpm" | "repaint"
     ddpm_steps: int = 1000               # per stage, schedule == "ddpm"
     ddim_steps: int = 50                 # per stage, schedule == "ddim"
     ddim_eta: float = 0.0                # schedule == "ddim": 0 = deterministic DDIM, 1 = DDPM-like noise
     dpm_steps: int = 20                  # per stage, schedule == "dpm"
     dpm_order: int = 2                   # schedule == "dpm": 1 (DDIM-like) or 2 (DPM-Solver++ 2M)
     dpm_algorithm: str = "dpmsolver++"   # schedule == "dpm": "dpmsolver++" (ODE) or "sde-dpmsolver++" (SDE)
+    repaint_steps: int = 250             # schedule == "repaint": N of RePaintScheduler.set_timesteps (diffusers' default)
+    repaint_eta: float = 0.0             # schedule == "repaint": DDIM eta of the steps
+    repaint_jump_length: int = 10        # schedule == "repaint": entries noised back up per jump
+    repaint_jump_n_sample: int = 10      # schedule == "repaint": passes over each jump (1 = no resampling: DDIM-N)
     dense_masks: bool = False            # True: skip dedup, every slot valid (the dense-FLOP benchmark mode)
     ragged_masks: bool = False           # benchmark only: synthetic masks shaped like a trained model's output (random-init
                                          # weights never produce duplicates): 1/8..1/2 of the faces valid, 3..E/3 edges each
@@ -141,8 +146,9 @@ def per_sample_seeds(cfg: CascadeConfig) -> Optional[List[int]]:
 
 
 def check_schedule(cfg: CascadeConfig) -> None:
-    """raises ValueError on out-of-range DDIM settings (ddim_steps outside [1, 1000], ddim_eta < 0) and DPM settings
-    (dpm_steps outside [1, 1000], dpm_order not 1 or 2, an unknown dpm_algorithm)"""
+    """raises ValueError on out-of-range DDIM settings (ddim_steps outside [1, 1000], ddim_eta < 0), DPM settings
+    (dpm_steps outside [1, 1000], dpm_order not 1 or 2, an unknown dpm_algorithm) and RePaint settings (repaint_steps
+    outside [1, 1000], repaint_eta < 0, repaint_jump_length or repaint_jump_n_sample < 1)"""
     if cfg.schedule == "ddim":
         if not 1 <= int(cfg.ddim_steps) <= 1000:
             raise ValueError(f"CascadeConfig.ddim_steps must be in [1, 1000], got {cfg.ddim_steps}")
@@ -155,6 +161,14 @@ def check_schedule(cfg: CascadeConfig) -> None:
             raise ValueError(f"CascadeConfig.dpm_order must be 1 or 2, got {cfg.dpm_order}")
         if cfg.dpm_algorithm not in DPM_ALGORITHMS:
             raise ValueError(f"CascadeConfig.dpm_algorithm must be one of {DPM_ALGORITHMS}, got {cfg.dpm_algorithm!r}")
+    if cfg.schedule == "repaint":
+        if not 1 <= int(cfg.repaint_steps) <= 1000:
+            raise ValueError(f"CascadeConfig.repaint_steps must be in [1, 1000], got {cfg.repaint_steps}")
+        if not float(cfg.repaint_eta) >= 0.0:
+            raise ValueError(f"CascadeConfig.repaint_eta must be >= 0, got {cfg.repaint_eta}")
+        for f in ("repaint_jump_length", "repaint_jump_n_sample"):
+            if not int(getattr(cfg, f)) >= 1:
+                raise ValueError(f"CascadeConfig.{f} must be >= 1, got {getattr(cfg, f)}")
 
 
 @dataclass
@@ -191,8 +205,9 @@ def check_completion(cfg: CascadeConfig, known: Completion) -> torch.Tensor:
     """raises on a Completion `cfg` cannot run (host checks only; Cascade.run adds the duplicate-face check on the
     device); returns n_faces as a CPU int64 tensor"""
     if cfg.schedule == "reference":
-        raise NotImplementedError("completion needs schedule='ddpm', 'ddim' or 'dpm': PNDM's Runge-Kutta steps advance from a "
-                                  "sample stored earlier (cur_sample), so known tokens cannot be replaced between them")
+        raise NotImplementedError("completion needs schedule='ddpm', 'ddim', 'dpm' or 'repaint': PNDM's Runge-Kutta "
+                                  "steps advance from a sample stored earlier (cur_sample), so known tokens cannot be "
+                                  "replaced between them")
     if cfg.dense_masks or cfg.ragged_masks:
         raise ValueError("completion runs the de-duplication; dense_masks and ragged_masks are benchmark modes")
     B, E = cfg.batch_size, cfg.num_edges
@@ -282,6 +297,8 @@ class Cascade:
                                   beta_start=0.0001, beta_end=0.02, clip_sample=True, clip_sample_range=3,
                                   set_alpha_to_one=True)
         self.dpm = self._dpm_scheduler(2, "dpmsolver++")
+        self.repaint = RePaintScheduler(num_train_timesteps=1000, beta_schedule="linear", beta_start=0.0001,
+                                        beta_end=0.02, clip_sample=True, clip_sample_range=3)
 
     @staticmethod
     def _dpm_scheduler(order: int, algorithm: str) -> DPMSolverMultistepScheduler:
@@ -476,15 +493,126 @@ class Cascade:
         nz = noise_fn(k, x.shape).to(self.device) if (noise_fn is not None and int(t) > 0) else None
         return sched.step(pred, t, x, generator=gen, noise=nz, **cf).prev_sample
 
+    # ------------------------------------------------------------------ RePaint: steps and undo steps in list order
+    def _loop_repaint(self, cfg: CascadeConfig, sched: RePaintScheduler, x, fwd, on_step=None, noise_fn=None, known=None,
+                      unoise_fn=None):
+        """The loop of diffusers' RePaint pipeline over sched.timesteps: a step entry runs fwd and the fused RePaint step
+        against the known tokens of x's current shape (known: {slots: (values, token mask)}, or None); an undo entry
+        noises x back up from the previous entry.  on_step(t, x) is probed at every entry, so the late face-count increase
+        happens once, at the first t <= 249; later jumps back above 249 keep the doubled shape.  noise_fn(k, shape) /
+        unoise_fn(k, (n, *shape)) -> explicit noise of entry k (parity runs); without them a launch-bound stage runs as
+        two replayed CUDA graphs per segment."""
+        ts = sched.timesteps
+        ents = repaint_entries(ts)
+        dev = self.device
+        tokens = x[0].numel() // x.shape[-1] * x.shape[0] * (2 if cfg.use_cf else 1)
+        if noise_fn is None and unoise_fn is None and len(ents) > 0 and self._use_graph(cfg, len(ents), tokens):
+            tables = (sched.coefficient_table().to(dev), sched.undo_table().to(dev),
+                      ts.to(device=dev, dtype=torch.int64).contiguous())
+            lo = 0
+            while lo < len(ents):
+                if on_step is not None:
+                    x = on_step(int(ts[lo]), x)
+                hi = lo + 1
+                while hi < len(ents) and (on_step is None or on_step(int(ts[hi]), x).shape == x.shape):
+                    hi += 1
+                x = self._loop_graph_repaint(cfg, sched, ents, lo, hi, x, fwd, known, tables)
+                lo = hi
+            return x
+        ts_dev = ts.to(dev)
+        for k, (is_step, t) in enumerate(ents):
+            if on_step is not None:
+                x = on_step(int(ts[k]), x)
+            B = x.shape[0]
+            if is_step:
+                kn, km = known[x.shape[1]] if known is not None else (None, None)
+                nz = noise_fn(k, x.shape).to(dev) if noise_fn is not None else None
+                t_dev = ts_dev[k:k + 1]
+                if cfg.use_cf:
+                    pred = fwd(torch.cat([x, x], 0), t_dev)
+                    x = sched.step(pred[:B], t, x, kn, km, noise=nz, model_output_uncond=pred[B:],
+                                   guidance_w=cfg.guidance_w).prev_sample
+                else:
+                    x = sched.step(fwd(x, t_dev), t, x, kn, km, noise=nz).prev_sample
+            else:
+                nz = unoise_fn(k, (sched.undo_transitions,) + tuple(x.shape)).to(dev) if unoise_fn is not None else None
+                x = sched.undo_step(x, t, noise=nz, out=x)
+        return x
+
+    def _loop_graph_repaint(self, cfg, sched, ents, lo, hi, x, fwd, known, tables):
+        """entries lo..hi-1 of a stage's RePaint list (one shape) as two captured bodies sharing the entry counter `step`
+        and t_cur: advance -> forward -> bg_repaint_step_tab, and advance -> bg_repaint_undo_tab, replayed in list order.
+        The counter runs over the whole list (it starts at lo - 1), so the tables (step coefficients, undo coefficients,
+        timesteps) are those of the whole stage and the noise counters are the eager loop's."""
+        dev = self.device
+        lib = _ffi.lib()
+        coef, utab, ts = tables
+        T = len(ents)
+        B = x.shape[0]
+        xb = x.detach().float().contiguous().clone()
+        n = xb.numel()
+        step = torch.full((1,), lo - 1, dtype=torch.int32, device=dev)
+        t_cur = torch.zeros(1, dtype=torch.int64, device=dev)
+        keys = sched.sample_key_tensor(B, dev) if sched.per_sample_noise else None
+        s3, s4 = (0, 0) if keys is not None else (sched.repaint_seed(3), sched.repaint_seed(4))
+        clip = float(sched.config.clip_sample_range) if sched.config.clip_sample else 0.0
+        kn, km = known[xb.shape[1]] if known is not None else (None, None)
+        nt = sched.undo_transitions
+
+        def advance(st):
+            _ffi.check(lib.bg_step_advance(ts.data_ptr(), T, step.data_ptr(), t_cur.data_ptr(), st), "bg_step_advance")
+
+        def step_body():
+            st = _ffi.current_stream()
+            advance(st)
+            pred = fwd(torch.cat([xb, xb], 0) if cfg.use_cf else xb, t_cur)
+            pc = pred[:B] if cfg.use_cf else pred
+            pu = pred[B:] if cfg.use_cf else None
+            _ffi.check(lib.bg_repaint_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(),
+                                               xb.data_ptr(), _ffi.ptr(kn), _ffi.ptr(km), xb.shape[-1], s3,
+                                               _ffi.ptr(keys), n // B, n, coef.data_ptr(), step.data_ptr(), clip, st),
+                       "bg_repaint_step_tab")
+
+        def undo_body():
+            st = _ffi.current_stream()
+            advance(st)
+            _ffi.check(lib.bg_repaint_undo_tab(xb.data_ptr(), n, nt, s4, _ffi.ptr(keys), n // B, utab.data_ptr(),
+                                               step.data_ptr(), st), "bg_repaint_undo_tab")
+
+        # warm-up outside the capture (packs the weights, allocates the workspace), then rewind the state it touched
+        x0 = xb.clone()
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side):
+            step_body()
+        torch.cuda.current_stream(dev).wait_stream(side)
+        xb.copy_(x0)
+        step.fill_(lo - 1)
+        kinds = [ents[k][0] for k in range(lo, hi)]
+        graphs, per_replay = {}, {}
+        for is_step, body in ((True, step_body), (False, undo_body)):
+            if is_step in kinds:
+                g = torch.cuda.CUDAGraph()
+                l0 = lib.bg_launch_count()
+                with torch.cuda.graph(g):
+                    body()
+                graphs[is_step], per_replay[is_step] = g, lib.bg_launch_count() - l0
+        for is_step in kinds:
+            graphs[is_step].replay()
+        for is_step in graphs:
+            _ffi.note_replay(per_replay[is_step], kinds.count(is_step))
+        self.last_graph_steps = getattr(self, "last_graph_steps", 0) + (hi - lo)
+        return xb
+
     _STAGE_ID = {"surfPos": 0, "surfZ": 1, "edgePos": 2, "edgeZV": 3}
 
     def _stage(self, cfg, x, fwd, label2, gen, hybrid_ddpm_tail: bool, on_step=None, noise_fn=None, name="surfPos",
-               known=None, rnoise_fn=None):
+               known=None, rnoise_fn=None, unoise_fn=None):
         seeds = getattr(self, "_sample_seeds", None)
         if cfg.schedule == "dpm" and (self.dpm.config.solver_order, self.dpm.config.algorithm_type) != \
                 (cfg.dpm_order, cfg.dpm_algorithm):
             self.dpm = self._dpm_scheduler(cfg.dpm_order, cfg.dpm_algorithm)
-        noisy = {"ddim": self.ddim, "dpm": self.dpm}.get(cfg.schedule, self.ddpm)
+        noisy = {"ddim": self.ddim, "dpm": self.dpm, "repaint": self.repaint}.get(cfg.schedule, self.ddpm)
         if seeds is not None:
             noisy.set_sample_keys(sample_seeds=seeds, stage=self._STAGE_ID[name])
         else:
@@ -495,6 +623,10 @@ class Cascade:
         if cfg.schedule == "dpm":
             self.dpm.set_timesteps(cfg.dpm_steps)
             return self._loop(cfg, self.dpm, self.dpm.timesteps, x, fwd, label2, gen, on_step, noise_fn, known, rnoise_fn)
+        if cfg.schedule == "repaint":
+            self.repaint.eta = float(cfg.repaint_eta)
+            self.repaint.set_timesteps(cfg.repaint_steps, cfg.repaint_jump_length, cfg.repaint_jump_n_sample)
+            return self._loop_repaint(cfg, self.repaint, x, fwd, on_step, noise_fn, known, unoise_fn)
         if cfg.schedule == "ddpm":
             self.ddpm.set_timesteps(cfg.ddpm_steps)
             return self._loop(cfg, self.ddpm, self.ddpm.timesteps, x, fwd, label2, gen, on_step, noise_fn, known, rnoise_fn)
@@ -556,7 +688,7 @@ class Cascade:
     # ------------------------------------------------------------------ the cascade
     @torch.no_grad()
     def run(self, cfg: CascadeConfig, init_noise: Optional[Dict[str, torch.Tensor]] = None, step_noise=None,
-            known: Optional[Completion] = None, replace_noise=None):
+            known: Optional[Completion] = None, replace_noise=None, undo_noise=None):
         """step_noise(stage_name, k, shape) -> tensor: explicit DDPM / DDIM / DPM step noise of step k (parity runs; DDPM
         draws it at t > 0, DDIM on every step when ddim_eta > 0, DPM on every step of "sde-dpmsolver++"); default = in-kernel
         Philox
@@ -566,7 +698,11 @@ class Cascade:
         known: a Completion (schedules "ddpm", "ddim" and "dpm"): every stage that has known tokens replaces them before its
         first step and after every step with the known values noised to the step's level, so the rest is generated
         around them; the known parts come out as given, bit for bit.  replace_noise(stage_name, k, shape) -> tensor:
-        explicit noise of that replacement (k = -1 before the first step; parity runs), mirroring step_noise."""
+        explicit noise of that replacement (k = -1 before the first step; parity runs), mirroring step_noise.
+        schedule "repaint": step_noise(stage_name, k, shape) is the one z of the step at list entry k (drawn at every
+        step); undo_noise(stage_name, k, (n, *shape)) the normals of the undo step at entry k.  Known tokens are kept by
+        the RePaint step itself (no separate replacement: replace_noise is not used), and known=None is DDIM with
+        resampling."""
         check_schedule(cfg)
         n_known = check_completion(cfg, known) if known is not None else None
         seeds = per_sample_seeds(cfg)
@@ -582,6 +718,8 @@ class Cascade:
         self._noise_key = (int(cfg.seed), rank)
         nf = (lambda name: (lambda k, shape: step_noise(name, k, shape))) if step_noise is not None else (lambda name: None)
         rnf = (lambda name: (lambda k, shape: replace_noise(name, k, shape))) if replace_noise is not None else \
+            (lambda name: None)
+        unf = (lambda name: (lambda k, shape: undo_noise(name, k, shape))) if undo_noise is not None else \
             (lambda name: None)
         gen = None
         B, S0, E = cfg.batch_size, cfg.num_surfaces, cfg.num_edges
@@ -612,7 +750,8 @@ class Cascade:
         surfPos = noise("surfPos", (B, S0, 6))
         surfPos = self._stage(cfg, surfPos, lambda x, t: self.m["surfpos"](x, t, label2), label2, gen, True,
                               on_step=late_increase, noise_fn=nf("surfPos"), name="surfPos", known=kn.get("surfPos"),
-                              rnoise_fn=rnf("surfPos"))
+                              rnoise_fn=rnf("surfPos"),
+                              unoise_fn=unf("surfPos"))
         if not cfg.use_cf and surfPos.shape[1] == S0:
             surfPos = surfPos.repeat(1, 2, 1)
 
@@ -630,13 +769,15 @@ class Cascade:
         # STEP 1-3 surface latents (sample.py:189-202)
         surfZ = noise("surfZ", (B, S, 48))
         surfZ = self._stage(cfg, surfZ, lambda x, t: self.m["surfz"](x, t, sP, sM, label2), label2, gen, False,
-                            noise_fn=nf("surfZ"), name="surfZ", known=kn.get("surfZ"), rnoise_fn=rnf("surfZ"))
+                            noise_fn=nf("surfZ"), name="surfZ", known=kn.get("surfZ"), rnoise_fn=rnf("surfZ"),
+                            unoise_fn=unf("surfZ"))
         sZ = rep2(surfZ)
 
         # STEP 2-1 edge positions (sample.py:208-236)
         edgePos = noise("edgePos", (B, S, E, 6))
         edgePos = self._stage(cfg, edgePos, lambda x, t: self.m["edgepos"](x, t, sP, sZ, sM, label2), label2, gen, True,
-                              noise_fn=nf("edgePos"), name="edgePos", known=kn.get("edgePos"), rnoise_fn=rnf("edgePos"))
+                              noise_fn=nf("edgePos"), name="edgePos", known=kn.get("edgePos"), rnoise_fn=rnf("edgePos"),
+                              unoise_fn=unf("edgePos"))
 
         # STEP 2-2 duplicate edges per face (sample.py:242-261)
         if cfg.ragged_masks:
@@ -653,7 +794,8 @@ class Cascade:
         # STEP 2-3 edge latents + vertices (sample.py:267-286)
         edgeZV = noise("edgeZV", (B, S, E, 18))
         edgeZV = self._stage(cfg, edgeZV, lambda x, t: self.m["edgez"](x, t, eP, sP, sZ, eM, label2), label2, gen, False,
-                             noise_fn=nf("edgeZV"), name="edgeZV", known=kn.get("edgeZV"), rnoise_fn=rnf("edgeZV"))
+                             noise_fn=nf("edgeZV"), name="edgeZV", known=kn.get("edgeZV"), rnoise_fn=rnf("edgeZV"),
+                             unoise_fn=unf("edgeZV"))
         edgeZV = edgeZV.masked_fill(edgeM.unsqueeze(-1), 0.0)
         edge_z, edgeV = edgeZV[..., :12], edgeZV[..., 12:]
 

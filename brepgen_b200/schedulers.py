@@ -1,6 +1,6 @@
-"""Drop-in DDPMScheduler / PNDMScheduler with the diffusers 0.27 interface used by the reference, and DDIMScheduler and
-DPMSolverMultistepScheduler (diffusers' few-step samplers for the same epsilon-prediction models; not used by the
-reference).
+"""Drop-in DDPMScheduler / PNDMScheduler with the diffusers 0.27 interface used by the reference, DDIMScheduler and
+DPMSolverMultistepScheduler (diffusers' few-step samplers for the same epsilon-prediction models) and RePaintScheduler
+(diffusers' inpainting with resampling; none of these three is used by the reference).
 
 Call sites mirrored (all in the reference): constructors sample.py:101-117 and trainer.py:285-292;
 `set_timesteps(n)` + `.timesteps[...]` slicing sample.py:128-129,144-145; `.step(pred, t, x).prev_sample`
@@ -8,7 +8,7 @@ sample.py:137,153,202,222,236,282; `.add_noise(x, noise, t)` trainer.py:348; `.c
 
 Host side (this file): the beta / alphas_cumprod tables and the per-step scalar coefficients, computed with the same
 fp32 torch-CPU operations diffusers uses (SURVEY.md Appendix A.3/A.4).  Device side: ONE fused kernel per step
-(bg_ddpm_step / bg_ddim_step / bg_dpm_step / bg_pndm_step in csrc/sched.cu) instead of ~15 scalar-broadcast launches.  No CPU tensor path:
+(bg_ddpm_step / bg_ddim_step / bg_dpm_step / bg_repaint_step / bg_pndm_step in csrc/sched.cu) instead of ~15 scalar-broadcast launches.  No CPU tensor path:
 `step` on a CPU sample raises.
 """
 from __future__ import annotations
@@ -446,6 +446,244 @@ class DDIMScheduler(_NoiseStreams):
                                               float(self.config.clip_sample_range) if self.config.clip_sample else 0.0,
                                               int(bool(use_clipped_model_output)), _ffi.current_stream()), "bg_ddim_step")
         return SchedulerOutput(dst) if return_dict else (dst,)
+
+    def add_noise(self, original_samples, noise, timesteps):
+        return DDPMScheduler.add_noise(self, original_samples, noise, timesteps)
+
+    def __len__(self):
+        return self.config.num_train_timesteps
+
+
+def repaint_timesteps(num_inference_steps: int, jump_length: int, jump_n_sample: int,
+                      num_train_timesteps: int = 1000) -> np.ndarray:
+    """int64 timesteps of diffusers' RePaintScheduler.set_timesteps: N - 1 .. 0 in steps of one, with a jump back up by
+    jump_length after every jump_length-th index, jump_n_sample - 1 times each, scaled by num_train_timesteps // N"""
+    n = min(num_train_timesteps, int(num_inference_steps))
+    jumps = {j: jump_n_sample - 1 for j in range(0, n - jump_length, jump_length)}
+    t, ts = n, []
+    while t >= 1:
+        t -= 1
+        ts.append(t)
+        if jumps.get(t, 0) > 0:
+            jumps[t] -= 1
+            for _ in range(jump_length):
+                t += 1
+                ts.append(t)
+    return np.array(ts, dtype=np.int64) * (num_train_timesteps // n)
+
+
+def repaint_entries(timesteps):
+    """[(is_step, t)] of the RePaint loop over `timesteps` (diffusers' pipeline): an entry below the previous one is a
+    denoising step at t; any other is an undo_step from the previous entry t_last (the first entry is a step)"""
+    ts = [_as_int(t) for t in timesteps]
+    out, t_last = [], (ts[0] + 1 if ts else 0)
+    for t in ts:
+        out.append((True, t) if t < t_last else (False, t_last))
+        t_last = t
+    return out
+
+
+class RePaintScheduler(_NoiseStreams):
+    """diffusers 0.27 RePaintScheduler for epsilon-prediction models: DDIM-form steps that keep the known region at
+    q(x_prev | known), and undo steps that noise the whole sample back up so the generated part is denoised again around
+    the known part (Lugmayr et al. 2022).  One fused kernel per entry (bg_repaint_step / bg_repaint_undo); the per-step
+    scalars are those of DDIMScheduler (set_alpha_to_one), computed in fp32 torch as diffusers computes them.
+
+    mask: 1 / True = known, one value per token (sample.shape[:-1], or with a trailing 1), bool, uint8 or a float tensor
+    holding only 0 and 1 -- the kernel selects, it does not blend.  Extras over diffusers: `clip_sample_range` (diffusers
+    clips to +-1), `model_output_uncond` + `guidance_w`, `noise`, `out`, the noise streams of set_noise_seed /
+    set_sample_keys, and the coefficient tables of the graph form.  Keyed and in-kernel noise are counted by the entry
+    index of the current timestep list (reset by set_timesteps; step and undo_step each take one entry)."""
+
+    def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.0001, beta_end: float = 0.02,
+                 beta_schedule: str = "linear", eta: float = 0.0, trained_betas=None, clip_sample: bool = True,
+                 clip_sample_range: float = 1.0, prediction_type: str = "epsilon", **unused):
+        if trained_betas is not None or prediction_type != "epsilon":
+            raise NotImplementedError("only prediction_type='epsilon' and no trained_betas")
+        self.config = SimpleNamespace(num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
+                                      beta_schedule=beta_schedule, eta=eta, trained_betas=trained_betas,
+                                      clip_sample=clip_sample, clip_sample_range=clip_sample_range,
+                                      prediction_type=prediction_type)
+        self._ddim = DDIMScheduler(num_train_timesteps, beta_start, beta_end, beta_schedule, clip_sample=clip_sample,
+                                   set_alpha_to_one=True, clip_sample_range=clip_sample_range)
+        self.betas, self.alphas_cumprod = self._ddim.betas, self._ddim.alphas_cumprod
+        self.eta = float(eta)
+        self.init_noise_sigma = 1.0
+        self.num_inference_steps = None
+        self.timesteps = torch.from_numpy(np.arange(0, num_train_timesteps)[::-1].copy().astype(np.int64))
+        self._entry = 0
+        self._undo_rows = {}
+        self._init_noise_streams()
+
+    def set_timesteps(self, num_inference_steps: int, jump_length: int = 10, jump_n_sample: int = 10, device=None):
+        n_train = self.config.num_train_timesteps
+        if num_inference_steps < 1 or jump_length < 1 or jump_n_sample < 1:
+            raise ValueError("num_inference_steps, jump_length and jump_n_sample must be positive")
+        ts = repaint_timesteps(num_inference_steps, jump_length, jump_n_sample, n_train)
+        n = min(n_train, num_inference_steps)
+        if len(ts) * (n_train // n) >= 2 ** 32:
+            raise ValueError(f"a list of {len(ts)} entries with {n_train // n} transitions per undo overflows the 32-bit "
+                             "noise counter")
+        self.num_inference_steps = n
+        self._ddim.set_timesteps(n)
+        self.timesteps = torch.from_numpy(ts)
+        self._entry = 0
+
+    def scale_model_input(self, sample, timestep=None):
+        return sample
+
+    @property
+    def undo_transitions(self) -> int:
+        """n = num_train_timesteps // num_inference_steps: the forward-diffusion transitions of one undo_step"""
+        self._need_timesteps()
+        return self.config.num_train_timesteps // self.num_inference_steps
+
+    def _need_timesteps(self):
+        if self.num_inference_steps is None:
+            raise ValueError("Number of inference steps is 'None', you need to run 'set_timesteps' after creating the "
+                             "scheduler")
+
+    def step_coefficients(self, t: int, eta: Optional[float] = None):
+        """(sqrt(1-abar_t), sqrt(abar_t), sqrt(abar_prev), c_dir, sigma, sqrt(1-abar_prev)) as Python floats: DDIM's
+        coefficients (abar_prev = 1 past the last step) and the noise level of the known part"""
+        self._need_timesteps()
+        sb, sa, sa_prev, c_dir, sigma = self._ddim.step_coefficients(int(t), self.eta if eta is None else eta)
+        return sb, sa, sa_prev, c_dir, sigma, float((1 - self._ddim._abar_prev(int(t))) ** 0.5)
+
+    def undo_coefficients(self, t_last: int) -> torch.Tensor:
+        """[n, 2] fp32 (CPU): (sqrt(1 - beta), sqrt(beta)) of transitions t_last .. t_last + n - 1, as diffusers computes
+        them"""
+        n = self.undo_transitions
+        if not 0 <= t_last <= self.config.num_train_timesteps - n:
+            raise ValueError(f"undo_step: timestep {t_last} + {n} transitions leaves the training range")
+        rows = [(float((1 - self.betas[t_last + i]) ** 0.5), float(self.betas[t_last + i] ** 0.5)) for i in range(n)]
+        return torch.tensor(rows, dtype=torch.float32)
+
+    def coefficient_table(self, timesteps=None, eta: Optional[float] = None) -> torch.Tensor:
+        """[len(timesteps), 6] fp32 (CPU): step_coefficients of every step entry of a RePaint loop (default: the whole
+        list), zero rows at undo entries -- the device table bg_repaint_step_tab indexes with the entry counter"""
+        ents = repaint_entries(self.timesteps if timesteps is None else timesteps)
+        rows = [self.step_coefficients(t, eta) if is_step else (0.0,) * 6 for is_step, t in ents]
+        return torch.tensor(rows, dtype=torch.float32).reshape(-1, 6)
+
+    def undo_table(self, timesteps=None) -> torch.Tensor:
+        """[len(timesteps), n, 2] fp32 (CPU): undo_coefficients(t_last) of every undo entry, zero at step entries -- the
+        device table bg_repaint_undo_tab indexes with the entry counter"""
+        ents = repaint_entries(self.timesteps if timesteps is None else timesteps)
+        n = self.undo_transitions
+        rows = [torch.zeros(n, 2) if is_step else self.undo_coefficients(t) for is_step, t in ents]
+        return torch.stack(rows, 0) if rows else torch.zeros(0, n, 2)
+
+    def repaint_seed(self, domain: int) -> int:
+        """batch-mode key of the step (domain 3) or undo (domain 4) noise: mix_seed(step stream key, domain).  It never
+        reads or advances the (seed, offset) stream of the other steps."""
+        if self._philox_seed is None:
+            self._philox_seed = mix_seed(torch.initial_seed())
+        return mix_seed(self._philox_seed, domain)
+
+    def _noise_source(self, batch, device, domain):
+        if self._sample_seeds is not None:
+            return 0, self.sample_key_tensor(batch, device)
+        return self.repaint_seed(domain), None
+
+    def _next_entry(self) -> int:
+        k = self._entry
+        self._entry += 1
+        return k
+
+    @staticmethod
+    def token_mask(mask: torch.Tensor, sample: torch.Tensor) -> torch.Tensor:
+        """the uint8 token mask (sample.shape[:-1]) of a step's `mask`; ValueError on another shape or a float value
+        other than 0 and 1"""
+        shp = tuple(sample.shape[:-1])
+        m = mask
+        if tuple(m.shape) == shp + (1,):
+            m = m[..., 0]
+        if tuple(m.shape) != shp:
+            raise ValueError(f"RePaintScheduler: mask must have shape {shp} (one value per token) or {shp + (1,)}, got "
+                             f"{tuple(mask.shape)}")
+        if m.dtype.is_floating_point:
+            if not bool(((m == 0) | (m == 1)).all()):
+                raise ValueError("RePaintScheduler: a float mask must hold only 0 and 1 (the step selects known or "
+                                 "generated values per token; it does not blend)")
+        elif m.dtype == torch.uint8:
+            return m.to(device=sample.device).contiguous()
+        elif m.dtype != torch.bool:
+            raise ValueError(f"RePaintScheduler: mask must be bool, uint8 or a 0/1 float tensor, got {m.dtype}")
+        return (m != 0).to(device=sample.device, dtype=torch.uint8).contiguous()
+
+    def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, original_image: Optional[torch.Tensor],
+             mask: Optional[torch.Tensor], generator=None, return_dict: bool = True,
+             model_output_uncond: Optional[torch.Tensor] = None, guidance_w: float = 0.0,
+             noise: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None):
+        """x at the previous timestep of diffusers' RePaint step: known tokens (mask = 1) at
+        sqrt(abar_prev) original_image + sqrt(1 - abar_prev) z, the others the DDIM update with eta = self.eta and the
+        variance term sigma z with the same z.  original_image = mask = None: nothing known.  z: `noise`, else `generator`
+        (one, or a list with one per batch element), else the per-sample streams of set_sample_keys (domain 3), else the
+        batch key repaint_seed(3), counted by the entry index.  pred_original_sample is not returned (None)."""
+        x, eps, eps_u, dst = _step_tensors("RePaintScheduler.step", model_output, sample, model_output_uncond, noise, out)
+        if (original_image is None) != (mask is None):
+            raise ValueError("RePaintScheduler.step: give original_image and mask together, or neither")
+        kn = m = None
+        if mask is not None:
+            if tuple(original_image.shape) != tuple(sample.shape):
+                raise RuntimeError(f"RePaintScheduler.step: original_image has shape {tuple(original_image.shape)}, "
+                                   f"sample has {tuple(sample.shape)}")
+            m = self.token_mask(mask, x)
+            kn = original_image.to(device=x.device, dtype=torch.float32).contiguous()
+        t = _as_int(timestep)
+        coefs = self.step_coefficients(t)
+        k = self._next_entry()
+        if noise is None and generator is not None:
+            noise = _generator_noise(x, generator)
+        if noise is not None:
+            noise = noise.to(device=x.device, dtype=torch.float32).contiguous()
+        n = x.numel()
+        seed, keys = self._noise_source(x.shape[0], x.device, 3)
+        clip = float(self.config.clip_sample_range) if self.config.clip_sample else 0.0
+        with torch.cuda.device(x.device):
+            _ffi.check(_ffi.lib().bg_repaint_step(eps.data_ptr(), _ffi.ptr(eps_u), float(guidance_w), x.data_ptr(),
+                                                 dst.data_ptr(), _ffi.ptr(kn), _ffi.ptr(m), x.shape[-1], _ffi.ptr(noise),
+                                                 seed, _ffi.ptr(keys), n // x.shape[0], k, n, *coefs, clip,
+                                                 _ffi.current_stream()), "bg_repaint_step")
+        return SchedulerOutput(dst) if return_dict else (dst,)
+
+    def undo_step(self, sample: torch.Tensor, timestep, generator=None, noise: Optional[torch.Tensor] = None,
+                  out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """sample noised by the n = num_train_timesteps // num_inference_steps forward transitions timestep ..
+        timestep + n - 1: x = sqrt(1 - beta) x + sqrt(beta) z, a fresh z per transition.  z: `noise` of shape
+        (n, *sample.shape), else n draws from `generator` in order (as diffusers draws them), else the per-sample streams
+        (domain 4), else the batch key repaint_seed(4), counted by the entry index.  out: destination, may be `sample`."""
+        _require_cuda(sample, "sample")
+        t_last = _as_int(timestep)
+        cf = self.undo_coefficients(t_last)
+        nt = cf.shape[0]
+        if noise is not None and tuple(noise.shape) != (nt,) + tuple(sample.shape):
+            raise RuntimeError(f"undo_step: noise has shape {tuple(noise.shape)}, want {(nt,) + tuple(sample.shape)}")
+        if out is not None and (out.dtype != torch.float32 or not out.is_contiguous() or out.device != sample.device or
+                                tuple(out.shape) != tuple(sample.shape)):
+            raise RuntimeError("undo_step: `out` must be a contiguous fp32 tensor of the sample's shape and device")
+        k = self._next_entry()
+        if out is None:
+            dst = sample.float().contiguous().clone()
+        else:
+            dst = out
+            if dst.data_ptr() != sample.data_ptr():
+                dst.copy_(sample)
+        if noise is None and generator is not None:
+            noise = torch.stack([_generator_noise(dst, generator).to(dst.device) for _ in range(nt)], 0)
+        if noise is not None:
+            noise = noise.to(device=dst.device, dtype=torch.float32).contiguous()
+        key = (t_last, nt, str(dst.device))
+        if key not in self._undo_rows:
+            self._undo_rows[key] = cf.to(dst.device)
+        n = dst.numel()
+        seed, keys = self._noise_source(dst.shape[0], dst.device, 4)
+        with torch.cuda.device(dst.device):
+            _ffi.check(_ffi.lib().bg_repaint_undo(dst.data_ptr(), n, nt, self._undo_rows[key].data_ptr(), _ffi.ptr(noise),
+                                                 seed, _ffi.ptr(keys), n // dst.shape[0], k, _ffi.current_stream()),
+                       "bg_repaint_undo")
+        return dst
 
     def add_noise(self, original_samples, noise, timesteps):
         return DDPMScheduler.add_noise(self, original_samples, noise, timesteps)

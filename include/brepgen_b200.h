@@ -157,7 +157,8 @@ int bg_step_advance(const int64_t* timesteps, int n_steps, int32_t* step, int64_
  * uint64 [n_samples], one Philox4x32-10 key per sample.  Element j of sample b is normal (j % 4) of the block with key
  * sample_keys[b] and counter (j / 4 as 64 bits, t, domain), Box-Muller as bg_ddpm_step; a block of 4 never straddles two
  * samples.  domain 0 = DDPM step noise at timestep t, domain 1 = initial noise (t = 0), domain 2 = known-token
- * replacement noise (bg_replace_known; t = the counter word t_ctr).  A sample's noise is therefore a
+ * replacement noise (bg_replace_known; t = the counter word t_ctr), domain 3 = RePaint step noise (bg_repaint_step; t = the
+ * list entry k), domain 4 = RePaint undo noise (bg_repaint_undo; t = k * n_trans + i).  A sample's noise is therefore a
  * function of its key alone, whatever the batch size, its position in the batch or the rank that runs it.
  * NULL sample_keys, per_sample <= 0 or n not a multiple of per_sample: BG_STATUS_BAD_ARG, nothing is launched. */
 /* out[b * per_sample + j] = normal j of sample b  (n_samples * per_sample fp32) */
@@ -240,6 +241,44 @@ int bg_replace_known(float* x, const float* known, const uint8_t* token_mask, in
 int bg_replace_known_tab(float* x, const float* known, const uint8_t* token_mask, int64_t n, int64_t per_token,
                          uint64_t seed, const uint64_t* sample_keys, int64_t per_sample, const int64_t* t_cur,
                          const float* coef_table, const int32_t* step, void* stream);
+/* RePaint step (diffusers RePaintScheduler.step, prediction_type "epsilon"; inpainting with resampling).  Every element
+ * of a token whose token_mask byte is zero gets the bg_ddim_step update, written with its expressions (bit-identical to
+ * bg_ddim_step with use_clipped_eps = 0 for the same noise):
+ *   out = sqrt_abar_prev*x0 + c_dir*eps + sigma*z,   x0 = clamp((x - sqrt_one_minus_abar*eps) / sqrt_abar, -clip, clip)
+ * (eps with the CFG combine of bg_ddpm_step); every element of a token whose byte is set gets the known part
+ *   out = sqrt_abar_prev*known + sqrt_one_minus_abar_prev*z   (fmaf; sqrt_abar_prev*known when the second is 0)
+ * with the SAME z.  Tokens are per_token consecutive elements.  known == NULL and token_mask == NULL: nothing known.
+ * z (drawn only when sigma != 0 or the group of 4 holds a known element): the explicit `noise` tensor if not NULL; else,
+ * when sample_keys != NULL, the per-sample streams at counter (j / 4, k, 3) (bg_randn_keyed(domain 3, k)), k = the entry's
+ * index in the stage's RePaint timestep list; else the batch key `seed`, the whole tensor counted as one sample.
+ * out may alias x.  BG_STATUS_BAD_ARG, launching nothing: NULL pointers, known without token_mask or the reverse,
+ * n not a multiple of per_token, (keyed) per_sample not a positive multiple of per_token dividing n, sqrt_abar <= 0,
+ * k outside 32 bits. */
+int bg_repaint_step(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
+                    const float* known, const uint8_t* token_mask, int64_t per_token, const float* noise, uint64_t seed,
+                    const uint64_t* sample_keys, int64_t per_sample, int64_t k, int64_t n, float sqrt_one_minus_abar,
+                    float sqrt_abar, float sqrt_abar_prev, float c_dir, float sigma, float sqrt_one_minus_abar_prev,
+                    float clip, void* stream);
+/* table-driven form for graph capture: coef_table[k][6] = (sqrt(1-abar_t), sqrt(abar_t), sqrt(abar_prev), c_dir, sigma,
+ * sqrt(1-abar_prev)) and the counter word k = *step (bg_step_advance over the whole RePaint list, so step and undo entries
+ * share the counter); no explicit noise.  Bit-identical to bg_repaint_step with the same coefficients, k and keys or seed. */
+int bg_repaint_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
+                        const float* known, const uint8_t* token_mask, int64_t per_token, uint64_t seed,
+                        const uint64_t* sample_keys, int64_t per_sample, int64_t n, const float* coef_table,
+                        const int32_t* step, float clip, void* stream);
+/* RePaint undo (diffusers RePaintScheduler.undo_step), in place: for i = 0..n_trans-1,
+ *   x = coef[2i]*x + coef[2i+1]*z_i        (coef[2i], coef[2i+1] = sqrt(1-beta), sqrt(beta) of transition i, device fp32)
+ * each product and the sum rounded on their own (the fp32 torch chain); x is read and written once.  z_i: the explicit
+ * `noise` tensor (n_trans, n) if not NULL; else, when sample_keys != NULL, the per-sample streams at counter
+ * (j / 4, k * n_trans + i, 4); else the batch key `seed`, the whole tensor counted as one sample.  BG_STATUS_BAD_ARG,
+ * launching nothing: NULL x / coef, n <= 0, n_trans <= 0, (keyed) per_sample not a positive divisor of n,
+ * k < 0 or (k + 1) * n_trans > 2^32. */
+int bg_repaint_undo(float* x, int64_t n, int32_t n_trans, const float* coef, const float* noise, uint64_t seed,
+                    const uint64_t* sample_keys, int64_t per_sample, int64_t k, void* stream);
+/* table-driven form: coef = coef_table + 2 * n_trans * k and the counter word k * n_trans + i, k = *step; no explicit
+ * noise.  Bit-identical to bg_repaint_undo with the same coefficients, k and keys or seed. */
+int bg_repaint_undo_tab(float* x, int64_t n, int32_t n_trans, uint64_t seed, const uint64_t* sample_keys,
+                        int64_t per_sample, const float* coef_table, const int32_t* step, void* stream);
 /* out = c_sample*x - c_eps*(w0*e0 + w1*e1 + w2*e2 + w3*e3)    (PNDM transfer + Adams-Bashforth / RK combination;
  * unused e_i may be NULL with w_i = 0) */
 int bg_pndm_step(const float* x, float* out, int64_t n, float c_sample, float c_eps, const float* e0, float w0,

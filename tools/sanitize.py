@@ -50,6 +50,11 @@ import test_gpu_completion as CO   # noqa: E402
 run("replace known", CO.test_kernel_matches_float64, 18, 13, "random")
 run("replace forms", CO.test_noise_forms_agree, 6, 7)
 run("replace bad args", CO.test_bad_arguments_are_rejected_and_launch_nothing)
+import test_gpu_repaint as RP   # noqa: E402
+run("repaint step", RP.test_step_matches_float64_and_ddim, 18, 13, 0.8, "random")
+run("repaint undo", RP.test_undo_is_the_fp32_chain_bit_for_bit, 50, 300)
+run("repaint forms", RP.test_noise_forms_agree, 6, 7)
+run("repaint bad args", RP.test_bad_arguments_are_rejected_and_launch_nothing)
 if what != "ops-no-res1":
     run("gemm", T.test_gemm, 128 * 170 + 5, 768, 1024, 0, 0, True, True, 0)   # persistent tiles wrap, residual epilogue
 if what == "all":
