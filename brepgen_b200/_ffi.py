@@ -44,12 +44,10 @@ SIGNATURES = {
     "bg_vae_posterior": (i32, [vp, vp, i32, i32, i32, vp, vp, vp]),
     "bg_vae_reconstruct_workspace_bytes": (sz, [vp, vp, i32]),
     "bg_vae_reconstruct": (i32, [vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, sz, vp]),
-    "bg_ddpm_step": (i32, [vp, vp, f32, vp, vp, vp, u64, u64, i64, f32, f32, f32, f32, f32, f32, vp]),
-    "bg_ddpm_step_tab": (i32, [vp, vp, f32, vp, vp, u64, u64, u64, i64, vp, vp, f32, vp]),
+    "bg_ddpm_step": (i32, [vp, vp, f32, vp, vp, vp, u64, u64, vp, i64, i64, i64, f32, f32, f32, f32, f32, f32, vp]),
+    "bg_ddpm_step_tab": (i32, [vp, vp, f32, vp, vp, u64, u64, u64, vp, i64, vp, i64, vp, vp, f32, vp]),
     "bg_step_advance": (i32, [vp, i32, vp, vp, vp]),
     "bg_randn_keyed": (i32, [vp, i64, i64, i32, i64, vp, vp]),
-    "bg_ddpm_step_keyed": (i32, [vp, vp, f32, vp, vp, vp, vp, i64, i64, i64, f32, f32, f32, f32, f32, f32, vp]),
-    "bg_ddpm_step_tab_keyed": (i32, [vp, vp, f32, vp, vp, vp, i64, vp, i64, vp, vp, f32, vp]),
     "bg_ddim_step": (i32, [vp, vp, f32, vp, vp, vp, u64, u64, vp, i64, i64, i64, f32, f32, f32, f32, f32, f32, i32, vp]),
     "bg_ddim_step_tab": (i32, [vp, vp, f32, vp, vp, u64, u64, u64, vp, i64, vp, i64, vp, vp, f32, i32, vp]),
     "bg_dpm_step": (i32, [vp, vp, f32, vp, vp, vp, vp, u64, u64, vp, i64, i64, i64, f32, f32, f32, f32, f32, f32, f32, f32,

@@ -35,83 +35,6 @@ __device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float& z0, fl
   z1 = rr * s;
 }
 
-struct DdpmP {
-  const float *eps_c, *eps_u, *x, *noise;
-  float* out;
-  long long n;
-  float w, sb, sa, clip, c_x0, c_x, sigma;
-  unsigned long long seed, offset;
-};
-
-__global__ void __launch_bounds__(256) ddpm_step_kernel(const DdpmP p) {
-  const long long n4 = (p.n + 3) / 4;
-  for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < n4; g += (long long)gridDim.x * blockDim.x) {
-    float z[4] = {0.f, 0.f, 0.f, 0.f};
-    if (p.sigma != 0.f && p.noise == nullptr) {
-      uint32_t r[4];
-      const unsigned long long ctr = p.offset + (unsigned long long)g;
-      philox4x32_10((uint32_t)ctr, (uint32_t)(ctr >> 32), 0u, 0u, (uint32_t)p.seed, (uint32_t)(p.seed >> 32), r);
-      box_muller(r[0], r[1], z[0], z[1]);
-      box_muller(r[2], r[3], z[2], z[3]);
-    }
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const long long i = g * 4 + j;
-      if (i >= p.n) break;
-      float e = p.eps_c[i];
-      if (p.eps_u) e = e * (1.f + p.w) - p.eps_u[i] * p.w;
-      const float xv = p.x[i];
-      float x0 = (xv - p.sb * e) / p.sa;
-      if (p.clip > 0.f) x0 = fminf(fmaxf(x0, -p.clip), p.clip);
-      float o = p.c_x0 * x0 + p.c_x * xv;
-      if (p.sigma != 0.f) o += p.sigma * (p.noise ? p.noise[i] : z[j]);
-      p.out[i] = o;
-    }
-  }
-}
-
-// Table-driven form for CUDA-graph replay: nothing step-specific is a kernel argument.  The coefficients of step k live in
-// coef[k][0..4] = (sqrt(1-abar_t), sqrt(abar_t), c_x0, c_x, sigma), k = *step is a device counter that bg_step_advance moves
-// on once per step, and the Philox counter starts at offset0 + k * offset_stride.
-struct DdpmTabP {
-  const float *eps_c, *eps_u, *x;
-  float* out;
-  long long n;
-  float w, clip;
-  const float* coef;
-  const int* step;
-  unsigned long long seed, offset0, offset_stride;
-};
-__global__ void __launch_bounds__(256) ddpm_step_tab_kernel(const DdpmTabP p) {
-  const int k = *p.step;
-  const float* cf = p.coef + 5 * (long long)k;
-  const float sb = cf[0], sa = cf[1], c_x0 = cf[2], c_x = cf[3], sigma = cf[4];
-  const unsigned long long offset = p.offset0 + (unsigned long long)k * p.offset_stride;
-  const long long n4 = (p.n + 3) / 4;
-  for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < n4; g += (long long)gridDim.x * blockDim.x) {
-    float z[4] = {0.f, 0.f, 0.f, 0.f};
-    if (sigma != 0.f) {
-      uint32_t r[4];
-      const unsigned long long ctr = offset + (unsigned long long)g;
-      philox4x32_10((uint32_t)ctr, (uint32_t)(ctr >> 32), 0u, 0u, (uint32_t)p.seed, (uint32_t)(p.seed >> 32), r);
-      box_muller(r[0], r[1], z[0], z[1]);
-      box_muller(r[2], r[3], z[2], z[3]);
-    }
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const long long i = g * 4 + j;
-      if (i >= p.n) break;
-      float e = p.eps_c[i];
-      if (p.eps_u) e = e * (1.f + p.w) - p.eps_u[i] * p.w;
-      const float xv = p.x[i];
-      float x0 = (xv - sb * e) / sa;
-      if (p.clip > 0.f) x0 = fminf(fmaxf(x0, -p.clip), p.clip);
-      float o = c_x0 * x0 + c_x * xv;
-      if (sigma != 0.f) o += sigma * z[j];
-      p.out[i] = o;
-    }
-  }
-}
 // Per-sample noise streams: element j of sample b is normal (j % 4) of Philox4x32-10 with key keys[b] and counter
 // (j / 4 as 64 bits, t, domain); domain 0 = DDPM step noise at timestep t, 1 = initial noise (t = 0).  A group of 4 never
 // straddles two samples (the last group of a sample uses its first per_sample % 4 normals), so a sample's noise does not
@@ -146,33 +69,50 @@ __global__ void __launch_bounds__(256) randn_keyed_kernel(const RandnKeyedP p) {
   }
 }
 
-// The DDPM update of ddpm_step_kernel with per-sample noise: the expressions are written exactly as there, so the keyed
-// step with noise == NULL is bit-identical to bg_ddpm_step fed the tensor bg_randn_keyed(domain 0, t) writes.
-// Table form (coef != NULL): coefficients from coef[*step], timestep from *t_cur, as ddpm_step_tab_kernel.
-struct DdpmKeyedP {
+// The four normals the DDPM, DDIM and DPM-Solver++ steps add to group q of sample b: the per-sample stream of keys[b] at
+// timestep t (domain 0) when keys != NULL, else the batch stream (seed, offset + q): the same Philox block under key seed
+// at counter (offset + q, 0, 0).  Without keys the whole tensor is one sample (per_sample = n), so q is the batch stream's
+// element group.
+__device__ __forceinline__ void step_normal4(const unsigned long long* keys, long long b, long long q, long long t,
+                                             unsigned long long seed, unsigned long long offset, float (&z)[4]) {
+  if (keys) keyed_normal4(keys[b], (unsigned long long)q, (uint32_t)t, 0u, z);
+  else keyed_normal4(seed, offset + (unsigned long long)q, 0u, 0u, z);
+}
+
+// DDPM step (diffusers 0.27 DDPMScheduler.step, epsilon prediction, fixed_small variance), per element:
+//   e = e*(1+w) - eu*w;  x0 = (x - sb*e) / sa, clamped to +-clip;  out = c_x0*x0 + c_x*x [+ sigma*z].
+// Every rounding is spelled out (one FMA each for e, x - sb*e, c_x*x + c_x0*x0 and + sigma*z), so that no compiler
+// contraction can move a bit of a sample.  Noise (only when sigma != 0): explicit `noise`, else step_normal4.  Table
+// form (coef != NULL): coefficients (sb, sa, c_x0, c_x, sigma) from coef[*step], t from *t_cur and the batch-stream
+// offset offset + k * offset_stride.
+struct DdpmP {
   const float *eps_c, *eps_u, *x, *noise;
   float* out;
   long long n, per_sample;
-  float w, sb, sa, clip, c_x0, c_x, sigma;
+  float w, sb, sa, c_x0, c_x, sigma, clip;
   const unsigned long long* keys;
   long long t;
+  unsigned long long seed, offset, offset_stride;
   const float* coef;
   const int* step;
   const long long* t_cur;
 };
-__global__ void __launch_bounds__(256) ddpm_step_keyed_kernel(const DdpmKeyedP p) {
+__global__ void __launch_bounds__(256) ddpm_step_kernel(const DdpmP p) {
   float sb = p.sb, sa = p.sa, c_x0 = p.c_x0, c_x = p.c_x, sigma = p.sigma;
   long long t = p.t;
+  unsigned long long offset = p.offset;
   if (p.coef) {
-    const float* cf = p.coef + 5 * (long long)*p.step;
+    const int k = *p.step;
+    const float* cf = p.coef + 5 * (long long)k;
     sb = cf[0]; sa = cf[1]; c_x0 = cf[2]; c_x = cf[3]; sigma = cf[4];
-    t = *p.t_cur;
+    if (p.t_cur) t = *p.t_cur;
+    offset += (unsigned long long)k * p.offset_stride;
   }
   const long long gps = (p.per_sample + 3) / 4, ng = (p.n / p.per_sample) * gps;
   for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += (long long)gridDim.x * blockDim.x) {
-    const long long b = g / gps, q = g - b * gps;
+    const long long b = p.keys ? g / gps : 0, q = g - b * gps;   // without keys: one sample, no division
     float z[4] = {0.f, 0.f, 0.f, 0.f};
-    if (sigma != 0.f && p.noise == nullptr) keyed_normal4(p.keys[b], (unsigned long long)q, (uint32_t)t, 0u, z);
+    if (sigma != 0.f && p.noise == nullptr) step_normal4(p.keys, b, q, t, p.seed, offset, z);
     const long long base = b * p.per_sample;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -180,12 +120,12 @@ __global__ void __launch_bounds__(256) ddpm_step_keyed_kernel(const DdpmKeyedP p
       if (js >= p.per_sample) break;
       const long long i = base + js;
       float e = p.eps_c[i];
-      if (p.eps_u) e = e * (1.f + p.w) - p.eps_u[i] * p.w;
+      if (p.eps_u) e = __fmaf_rn(e, 1.f + p.w, -__fmul_rn(p.eps_u[i], p.w));
       const float xv = p.x[i];
-      float x0 = (xv - sb * e) / sa;
+      float x0 = __fdiv_rn(__fmaf_rn(-sb, e, xv), sa);
       if (p.clip > 0.f) x0 = fminf(fmaxf(x0, -p.clip), p.clip);
-      float o = c_x0 * x0 + c_x * xv;
-      if (sigma != 0.f) o += sigma * (p.noise ? p.noise[i] : z[j]);
+      float o = __fmaf_rn(c_x, xv, __fmul_rn(c_x0, x0));
+      if (sigma != 0.f) o = __fmaf_rn(sigma, p.noise ? p.noise[i] : z[j], o);
       p.out[i] = o;
     }
   }
@@ -194,11 +134,9 @@ __global__ void __launch_bounds__(256) ddpm_step_keyed_kernel(const DdpmKeyedP p
 // DDIM step (diffusers 0.27 DDIMScheduler.step, epsilon prediction), diffusers' order of operations in fp32:
 //   x0 = (x - sb*e) / sa, clamped to +-clip;  e_dir = e, or (x - sa*x0) / sb with use_clipped_eps;
 //   out = sa_prev*x0 + c_dir*e_dir [+ sigma*z].
-// One kernel serves every form.  Noise: explicit `noise`, else per-sample keys (keyed_normal4, domain 0, timestep t: the
-// normals the keyed DDPM step draws at the same t), else the batch stream (seed, offset + element_group) of
-// ddpm_step_kernel.  Table form (coef != NULL): coefficients (sb, sa, sa_prev, c_dir, sigma) from coef[*step], t from
-// *t_cur and the batch-stream offset offset + k * offset_stride.  Without keys the whole tensor is one "sample"
-// (per_sample = n), so the group index is the batch stream's element group.
+// Noise (only when sigma != 0): explicit `noise`, else step_normal4, the normals the DDPM step draws at the same t.  Table
+// form (coef != NULL): coefficients (sb, sa, sa_prev, c_dir, sigma) from coef[*step], t from *t_cur and the batch-stream
+// offset offset + k * offset_stride.
 struct DdimP {
   const float *eps_c, *eps_u, *x, *noise;
   float* out;
@@ -227,17 +165,7 @@ __global__ void __launch_bounds__(256) ddim_step_kernel(const DdimP p) {
   for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += (long long)gridDim.x * blockDim.x) {
     const long long b = g / gps, q = g - b * gps;
     float z[4] = {0.f, 0.f, 0.f, 0.f};
-    if (sigma != 0.f && p.noise == nullptr) {
-      if (p.keys) {
-        keyed_normal4(p.keys[b], (unsigned long long)q, (uint32_t)t, 0u, z);
-      } else {
-        uint32_t r[4];
-        const unsigned long long ctr = offset + (unsigned long long)q;
-        philox4x32_10((uint32_t)ctr, (uint32_t)(ctr >> 32), 0u, 0u, (uint32_t)p.seed, (uint32_t)(p.seed >> 32), r);
-        box_muller(r[0], r[1], z[0], z[1]);
-        box_muller(r[2], r[3], z[2], z[3]);
-      }
-    }
+    if (sigma != 0.f && p.noise == nullptr) step_normal4(p.keys, b, q, t, p.seed, offset, z);
     const long long base = b * p.per_sample;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -293,17 +221,7 @@ __global__ void __launch_bounds__(256) dpm_step_kernel(const DpmP p) {
   for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += (long long)gridDim.x * blockDim.x) {
     const long long b = g / gps, q = g - b * gps;
     float z[4] = {0.f, 0.f, 0.f, 0.f};
-    if (c_z != 0.f && p.noise == nullptr) {
-      if (p.keys) {
-        keyed_normal4(p.keys[b], (unsigned long long)q, (uint32_t)t, 0u, z);
-      } else {
-        uint32_t r[4];
-        const unsigned long long ctr = offset + (unsigned long long)q;
-        philox4x32_10((uint32_t)ctr, (uint32_t)(ctr >> 32), 0u, 0u, (uint32_t)p.seed, (uint32_t)(p.seed >> 32), r);
-        box_muller(r[0], r[1], z[0], z[1]);
-        box_muller(r[2], r[3], z[2], z[3]);
-      }
-    }
+    if (c_z != 0.f && p.noise == nullptr) step_normal4(p.keys, b, q, t, p.seed, offset, z);
     // the group's loads first, then the math and the stores: no load waits behind a store it might alias
     const long long i0 = b * p.per_sample + q * 4;
     const int cnt = (int)min(4ll, p.per_sample - q * 4);
@@ -331,6 +249,22 @@ __global__ void __launch_bounds__(256) dpm_step_kernel(const DpmP p) {
       }
     }
   }
+}
+
+// known[j] = whether the token of element i0 + j (token = element / per_token) has its mask byte set, for j < cnt; returns
+// whether any is.  One division per group of 4: at most 4 mask bytes, usually 1 or 2 distinct.
+__device__ __forceinline__ bool known_flags(const unsigned char* mask, long long i0, long long per_token, int cnt,
+                                            bool (&known)[4]) {
+  long long tok = i0 / per_token, r = i0 - tok * per_token;
+  bool any = false;
+#pragma unroll
+  for (int j = 0; j < 4; ++j)
+    if (j < cnt) {
+      known[j] = mask[tok] != 0;
+      any |= known[j];
+      if (++r == per_token) { ++tok; r = 0; }
+    }
+  return any;
 }
 
 // Known-token replacement (B-rep completion): x[i] = sa*known[i] + sb*z for every element of a token whose mask byte is
@@ -364,18 +298,8 @@ __global__ void __launch_bounds__(256) replace_known_kernel(const ReplaceP p) {
     const long long b = g / gps, q = g - b * gps;
     const long long base = b * p.per_sample, js0 = q * 4;
     const int cnt = (int)min(4ll, p.per_sample - js0);
-    // tokens of the group's elements (one division per group): at most 4 mask bytes, usually 1 or 2 distinct
-    long long tok = (base + js0) / p.per_token, r = base + js0 - tok * p.per_token;
     bool known[4] = {false, false, false, false};
-    bool any = false;
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-      if (j < cnt) {
-        known[j] = p.mask[tok] != 0;
-        any |= known[j];
-        if (++r == p.per_token) { ++tok; r = 0; }
-      }
-    if (!any) continue;
+    if (!known_flags(p.mask, base + js0, p.per_token, cnt, known)) continue;
     float z[4] = {0.f, 0.f, 0.f, 0.f};
     if (p.noise == nullptr) keyed_normal4(p.keys ? p.keys[b] : p.seed, (unsigned long long)q, (uint32_t)t, 2u, z);
 #pragma unroll
@@ -423,17 +347,7 @@ __global__ void __launch_bounds__(256) repaint_step_kernel(const RepaintP p) {
     const long long base = b * p.per_sample, js0 = q * 4;
     const int cnt = (int)min(4ll, p.per_sample - js0);
     bool known[4] = {false, false, false, false};
-    bool any = false;
-    if (p.mask) {   // tokens of the group's elements, as replace_known_kernel: one division per group
-      long long tok = (base + js0) / p.per_token, r = base + js0 - tok * p.per_token;
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        if (j < cnt) {
-          known[j] = p.mask[tok] != 0;
-          any |= known[j];
-          if (++r == p.per_token) { ++tok; r = 0; }
-        }
-    }
+    const bool any = p.mask && known_flags(p.mask, base + js0, p.per_token, cnt, known);
     float z[4] = {0.f, 0.f, 0.f, 0.f};
     if ((sigma != 0.f || any) && p.noise == nullptr)
       keyed_normal4(p.keys ? p.keys[b] : p.seed, (unsigned long long)q, (uint32_t)k, 3u, z);
@@ -555,6 +469,17 @@ inline unsigned grid_for(long long work) {
   return (unsigned)blocks;
 }
 
+// Launches one of the grouped step kernels (one thread per group of 4 elements of a sample) over n / per_sample samples.
+// Without sample keys the whole tensor is one sample (per_sample = n), so a group is the batch stream's element group.
+template <class P>
+int launch_grouped(void (*kernel)(P), P& p, const uint64_t* sample_keys, int64_t per_sample, void* stream,
+                   const char* what) {
+  p.keys = reinterpret_cast<const unsigned long long*>(sample_keys);
+  p.per_sample = sample_keys ? per_sample : p.n;
+  kernel<<<grid_for((p.n / p.per_sample) * ((p.per_sample + 3) / 4)), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch(what);
+}
+
 }  // namespace
 }  // namespace bg
 
@@ -563,27 +488,33 @@ using namespace bg;
 extern "C" {
 
 int bg_ddpm_step(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
-                 const float* noise, uint64_t seed, uint64_t offset, int64_t n, float sqrt_one_minus_abar,
-                 float sqrt_abar, float clip, float c_x0, float c_x, float sigma, void* stream) {
+                 const float* noise, uint64_t seed, uint64_t offset, const uint64_t* sample_keys, int64_t per_sample,
+                 int64_t t, int64_t n, float sqrt_one_minus_abar, float sqrt_abar, float clip, float c_x0, float c_x,
+                 float sigma, void* stream) {
   BG_REQUIRE(eps_cond && x && out && n > 0, "ddpm_step: bad arguments");
+  BG_REQUIRE(!sample_keys || (per_sample > 0 && n % per_sample == 0),
+             "ddpm_step: n must be a positive multiple of per_sample");
+  BG_REQUIRE(t >= 0 && t <= 0xFFFFFFFFll, "ddpm_step: t must be a 32-bit unsigned value");
   BG_REQUIRE(sqrt_abar > 0.f, "ddpm_step: sqrt_abar must be positive");
-  DdpmP p;
+  DdpmP p = {};
   p.eps_c = eps_cond; p.eps_u = eps_uncond; p.x = x; p.noise = noise; p.out = out; p.n = n;
-  p.w = cfg_w; p.sb = sqrt_one_minus_abar; p.sa = sqrt_abar; p.clip = clip; p.c_x0 = c_x0; p.c_x = c_x; p.sigma = sigma;
-  p.seed = seed; p.offset = offset;
-  ddpm_step_kernel<<<grid_for((n + 3) / 4), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
-  return check_launch("ddpm_step_kernel launch");
+  p.w = cfg_w; p.sb = sqrt_one_minus_abar; p.sa = sqrt_abar; p.c_x0 = c_x0; p.c_x = c_x; p.sigma = sigma; p.clip = clip;
+  p.t = t; p.seed = seed; p.offset = offset;
+  return launch_grouped(ddpm_step_kernel, p, sample_keys, per_sample, stream, "ddpm_step_kernel launch");
 }
 
 int bg_ddpm_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out, uint64_t seed,
-                     uint64_t offset0, uint64_t offset_stride, int64_t n, const float* coef_table, const int32_t* step,
-                     float clip, void* stream) {
+                     uint64_t offset0, uint64_t offset_stride, const uint64_t* sample_keys, int64_t per_sample,
+                     const int64_t* t_cur, int64_t n, const float* coef_table, const int32_t* step, float clip,
+                     void* stream) {
   BG_REQUIRE(eps_cond && x && out && n > 0 && coef_table && step, "ddpm_step_tab: bad arguments");
-  DdpmTabP p;
+  BG_REQUIRE(!sample_keys || (t_cur && per_sample > 0 && n % per_sample == 0),
+             "ddpm_step_tab: keyed noise needs t_cur and n a positive multiple of per_sample");
+  DdpmP p = {};
   p.eps_c = eps_cond; p.eps_u = eps_uncond; p.x = x; p.out = out; p.n = n; p.w = cfg_w; p.clip = clip;
-  p.coef = coef_table; p.step = step; p.seed = seed; p.offset0 = offset0; p.offset_stride = offset_stride;
-  ddpm_step_tab_kernel<<<grid_for((n + 3) / 4), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
-  return check_launch("ddpm_step_tab_kernel launch");
+  p.seed = seed; p.offset = offset0; p.offset_stride = offset_stride;
+  p.coef = coef_table; p.step = step; p.t_cur = reinterpret_cast<const long long*>(t_cur);
+  return launch_grouped(ddpm_step_kernel, p, sample_keys, per_sample, stream, "ddpm_step_kernel launch");
 }
 
 int bg_randn_keyed(const uint64_t* sample_keys, int64_t n_samples, int64_t per_sample, int32_t domain, int64_t t, float* out,
@@ -596,47 +527,6 @@ int bg_randn_keyed(const uint64_t* sample_keys, int64_t n_samples, int64_t per_s
   p.n_samples = n_samples; p.per_sample = per_sample; p.domain = (uint32_t)domain; p.t = (uint32_t)t;
   randn_keyed_kernel<<<grid_for(n_samples * ((per_sample + 3) / 4)), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
   return check_launch("randn_keyed_kernel launch");
-}
-
-int bg_ddpm_step_keyed(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
-                       const float* noise, const uint64_t* sample_keys, int64_t per_sample, int64_t t, int64_t n,
-                       float sqrt_one_minus_abar, float sqrt_abar, float clip, float c_x0, float c_x, float sigma,
-                       void* stream) {
-  BG_REQUIRE(eps_cond && x && out && n > 0, "ddpm_step_keyed: bad arguments");
-  BG_REQUIRE(sample_keys != nullptr, "ddpm_step_keyed: sample_keys must not be NULL");
-  BG_REQUIRE(per_sample > 0 && n % per_sample == 0, "ddpm_step_keyed: n must be a positive multiple of per_sample");
-  BG_REQUIRE(t >= 0 && t <= 0xFFFFFFFFll, "ddpm_step_keyed: t must be a 32-bit unsigned value");
-  BG_REQUIRE(sqrt_abar > 0.f, "ddpm_step_keyed: sqrt_abar must be positive");
-  DdpmKeyedP p = {};
-  p.eps_c = eps_cond; p.eps_u = eps_uncond; p.x = x; p.noise = noise; p.out = out; p.n = n; p.per_sample = per_sample;
-  p.w = cfg_w; p.sb = sqrt_one_minus_abar; p.sa = sqrt_abar; p.clip = clip; p.c_x0 = c_x0; p.c_x = c_x; p.sigma = sigma;
-  p.keys = reinterpret_cast<const unsigned long long*>(sample_keys); p.t = t;
-  ddpm_step_keyed_kernel<<<grid_for((n / per_sample) * ((per_sample + 3) / 4)), 256, 0,
-                           reinterpret_cast<cudaStream_t>(stream)>>>(p);
-  return check_launch("ddpm_step_keyed_kernel launch");
-}
-
-int bg_ddpm_step_tab_keyed(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
-                           const uint64_t* sample_keys, int64_t per_sample, const int64_t* t_cur, int64_t n,
-                           const float* coef_table, const int32_t* step, float clip, void* stream) {
-  BG_REQUIRE(eps_cond && x && out && n > 0 && coef_table && step && t_cur, "ddpm_step_tab_keyed: bad arguments");
-  BG_REQUIRE(sample_keys != nullptr, "ddpm_step_tab_keyed: sample_keys must not be NULL");
-  BG_REQUIRE(per_sample > 0 && n % per_sample == 0, "ddpm_step_tab_keyed: n must be a positive multiple of per_sample");
-  DdpmKeyedP p = {};
-  p.eps_c = eps_cond; p.eps_u = eps_uncond; p.x = x; p.out = out; p.n = n; p.per_sample = per_sample;
-  p.w = cfg_w; p.clip = clip; p.keys = reinterpret_cast<const unsigned long long*>(sample_keys);
-  p.coef = coef_table; p.step = step; p.t_cur = reinterpret_cast<const long long*>(t_cur);
-  ddpm_step_keyed_kernel<<<grid_for((n / per_sample) * ((per_sample + 3) / 4)), 256, 0,
-                           reinterpret_cast<cudaStream_t>(stream)>>>(p);
-  return check_launch("ddpm_step_keyed_kernel launch");
-}
-
-static int launch_ddim(DdimP& p, const uint64_t* sample_keys, int64_t per_sample, void* stream) {
-  p.keys = reinterpret_cast<const unsigned long long*>(sample_keys);
-  p.per_sample = sample_keys ? per_sample : p.n;
-  ddim_step_kernel<<<grid_for((p.n / p.per_sample) * ((p.per_sample + 3) / 4)), 256, 0,
-                     reinterpret_cast<cudaStream_t>(stream)>>>(p);
-  return check_launch("ddim_step_kernel launch");
 }
 
 int bg_ddim_step(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
@@ -652,7 +542,7 @@ int bg_ddim_step(const float* eps_cond, const float* eps_uncond, float cfg_w, co
   p.eps_c = eps_cond; p.eps_u = eps_uncond; p.x = x; p.noise = noise; p.out = out; p.n = n;
   p.w = cfg_w; p.sb = sqrt_one_minus_abar; p.sa = sqrt_abar; p.sa_prev = sqrt_abar_prev; p.c_dir = c_dir; p.sigma = sigma;
   p.clip = clip; p.use_clipped_eps = use_clipped_eps != 0; p.t = t; p.seed = seed; p.offset = offset;
-  return launch_ddim(p, sample_keys, per_sample, stream);
+  return launch_grouped(ddim_step_kernel, p, sample_keys, per_sample, stream, "ddim_step_kernel launch");
 }
 
 int bg_ddim_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out, uint64_t seed,
@@ -666,15 +556,7 @@ int bg_ddim_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w
   p.eps_c = eps_cond; p.eps_u = eps_uncond; p.x = x; p.out = out; p.n = n; p.w = cfg_w; p.clip = clip;
   p.use_clipped_eps = use_clipped_eps != 0; p.seed = seed; p.offset = offset0; p.offset_stride = offset_stride;
   p.coef = coef_table; p.step = step; p.t_cur = reinterpret_cast<const long long*>(t_cur);
-  return launch_ddim(p, sample_keys, per_sample, stream);
-}
-
-static int launch_dpm(DpmP& p, const uint64_t* sample_keys, int64_t per_sample, void* stream) {
-  p.keys = reinterpret_cast<const unsigned long long*>(sample_keys);
-  p.per_sample = sample_keys ? per_sample : p.n;
-  dpm_step_kernel<<<grid_for((p.n / p.per_sample) * ((p.per_sample + 3) / 4)), 256, 0,
-                    reinterpret_cast<cudaStream_t>(stream)>>>(p);
-  return check_launch("dpm_step_kernel launch");
+  return launch_grouped(ddim_step_kernel, p, sample_keys, per_sample, stream, "ddim_step_kernel launch");
 }
 
 int bg_dpm_step(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out, float* hist,
@@ -691,7 +573,7 @@ int bg_dpm_step(const float* eps_cond, const float* eps_uncond, float cfg_w, con
   p.eps_c = eps_cond; p.eps_u = eps_uncond; p.x = x; p.noise = noise; p.out = out; p.hist = hist; p.n = n; p.w = cfg_w;
   p.alpha_s = alpha_s; p.sigma_s = sigma_s; p.c_x = c_x; p.c_0 = c_0; p.c_1 = c_1; p.inv_r0 = inv_r0; p.c_z = c_z;
   p.clip = clip; p.t = t; p.seed = seed; p.offset = offset;
-  return launch_dpm(p, sample_keys, per_sample, stream);
+  return launch_grouped(dpm_step_kernel, p, sample_keys, per_sample, stream, "dpm_step_kernel launch");
 }
 
 int bg_dpm_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out, float* hist,
@@ -704,15 +586,7 @@ int bg_dpm_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w,
   p.eps_c = eps_cond; p.eps_u = eps_uncond; p.x = x; p.out = out; p.hist = hist; p.n = n; p.w = cfg_w; p.clip = clip;
   p.seed = seed; p.offset = offset0; p.offset_stride = offset_stride;
   p.coef = coef_table; p.step = step; p.t_cur = reinterpret_cast<const long long*>(t_cur);
-  return launch_dpm(p, sample_keys, per_sample, stream);
-}
-
-static int launch_replace(ReplaceP& p, const uint64_t* sample_keys, int64_t per_sample, void* stream) {
-  p.keys = reinterpret_cast<const unsigned long long*>(sample_keys);
-  p.per_sample = sample_keys ? per_sample : p.n;
-  replace_known_kernel<<<grid_for((p.n / p.per_sample) * ((p.per_sample + 3) / 4)), 256, 0,
-                         reinterpret_cast<cudaStream_t>(stream)>>>(p);
-  return check_launch("replace_known_kernel launch");
+  return launch_grouped(dpm_step_kernel, p, sample_keys, per_sample, stream, "dpm_step_kernel launch");
 }
 
 int bg_replace_known(float* x, const float* known, const uint8_t* token_mask, int64_t n, int64_t per_token,
@@ -726,7 +600,7 @@ int bg_replace_known(float* x, const float* known, const uint8_t* token_mask, in
   ReplaceP p = {};
   p.x = x; p.known = known; p.noise = noise; p.mask = token_mask; p.n = n; p.per_token = per_token;
   p.sa = sqrt_abar; p.sb = sqrt_one_minus_abar; p.seed = seed; p.t = t_ctr;
-  return launch_replace(p, sample_keys, per_sample, stream);
+  return launch_grouped(replace_known_kernel, p, sample_keys, per_sample, stream, "replace_known_kernel launch");
 }
 
 int bg_replace_known_tab(float* x, const float* known, const uint8_t* token_mask, int64_t n, int64_t per_token,
@@ -739,15 +613,7 @@ int bg_replace_known_tab(float* x, const float* known, const uint8_t* token_mask
   ReplaceP p = {};
   p.x = x; p.known = known; p.mask = token_mask; p.n = n; p.per_token = per_token; p.seed = seed;
   p.coef = coef_table; p.step = step; p.t_cur = reinterpret_cast<const long long*>(t_cur);
-  return launch_replace(p, sample_keys, per_sample, stream);
-}
-
-static int launch_repaint(RepaintP& p, const uint64_t* sample_keys, int64_t per_sample, void* stream) {
-  p.keys = reinterpret_cast<const unsigned long long*>(sample_keys);
-  p.per_sample = sample_keys ? per_sample : p.n;
-  repaint_step_kernel<<<grid_for((p.n / p.per_sample) * ((p.per_sample + 3) / 4)), 256, 0,
-                        reinterpret_cast<cudaStream_t>(stream)>>>(p);
-  return check_launch("repaint_step_kernel launch");
+  return launch_grouped(replace_known_kernel, p, sample_keys, per_sample, stream, "replace_known_kernel launch");
 }
 
 int bg_repaint_step(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
@@ -767,7 +633,7 @@ int bg_repaint_step(const float* eps_cond, const float* eps_uncond, float cfg_w,
   p.eps_c = eps_cond; p.eps_u = eps_uncond; p.x = x; p.out = out; p.known = known; p.mask = token_mask; p.noise = noise;
   p.n = n; p.per_token = per_token; p.w = cfg_w; p.sb = sqrt_one_minus_abar; p.sa = sqrt_abar; p.sa_prev = sqrt_abar_prev;
   p.c_dir = c_dir; p.sigma = sigma; p.sb_prev = sqrt_one_minus_abar_prev; p.clip = clip; p.seed = seed; p.k = k;
-  return launch_repaint(p, sample_keys, per_sample, stream);
+  return launch_grouped(repaint_step_kernel, p, sample_keys, per_sample, stream, "repaint_step_kernel launch");
 }
 
 int bg_repaint_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
@@ -784,15 +650,7 @@ int bg_repaint_step_tab(const float* eps_cond, const float* eps_uncond, float cf
   RepaintP p = {};
   p.eps_c = eps_cond; p.eps_u = eps_uncond; p.x = x; p.out = out; p.known = known; p.mask = token_mask; p.n = n;
   p.per_token = per_token; p.w = cfg_w; p.clip = clip; p.seed = seed; p.coef = coef_table; p.step = step;
-  return launch_repaint(p, sample_keys, per_sample, stream);
-}
-
-static int launch_undo(UndoP& p, const uint64_t* sample_keys, int64_t per_sample, void* stream) {
-  p.keys = reinterpret_cast<const unsigned long long*>(sample_keys);
-  p.per_sample = sample_keys ? per_sample : p.n;
-  repaint_undo_kernel<<<grid_for((p.n / p.per_sample) * ((p.per_sample + 3) / 4)), 256, 0,
-                        reinterpret_cast<cudaStream_t>(stream)>>>(p);
-  return check_launch("repaint_undo_kernel launch");
+  return launch_grouped(repaint_step_kernel, p, sample_keys, per_sample, stream, "repaint_step_kernel launch");
 }
 
 int bg_repaint_undo(float* x, int64_t n, int32_t n_trans, const float* coef, const float* noise, uint64_t seed,
@@ -804,7 +662,7 @@ int bg_repaint_undo(float* x, int64_t n, int32_t n_trans, const float* coef, con
              "repaint_undo: the counter words k * n_trans + i must be 32-bit unsigned values");
   UndoP p = {};
   p.x = x; p.noise = noise; p.n = n; p.n_trans = n_trans; p.cf = coef; p.seed = seed; p.k = k;
-  return launch_undo(p, sample_keys, per_sample, stream);
+  return launch_grouped(repaint_undo_kernel, p, sample_keys, per_sample, stream, "repaint_undo_kernel launch");
 }
 
 int bg_repaint_undo_tab(float* x, int64_t n, int32_t n_trans, uint64_t seed, const uint64_t* sample_keys,
@@ -814,7 +672,7 @@ int bg_repaint_undo_tab(float* x, int64_t n, int32_t n_trans, uint64_t seed, con
              "repaint_undo_tab: n must be a positive multiple of per_sample");
   UndoP p = {};
   p.x = x; p.n = n; p.n_trans = n_trans; p.seed = seed; p.coef = coef_table; p.step = step;
-  return launch_undo(p, sample_keys, per_sample, stream);
+  return launch_grouped(repaint_undo_kernel, p, sample_keys, per_sample, stream, "repaint_undo_kernel launch");
 }
 
 int bg_step_advance(const int64_t* timesteps, int n_steps, int32_t* step, int64_t* t_cur, void* stream) {

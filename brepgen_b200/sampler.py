@@ -321,10 +321,11 @@ class Cascade:
         forward -> fused scheduler step (CFG combine, x0, clip, DDPM posterior mean or DDIM update, Philox noise) -- is
         captured ONCE and replayed len(timesteps) times: no per-step host work.  Nothing step-specific is a kernel argument:
         the timestep comes from a device scalar, the coefficients from a device table indexed by a device counter
-        (bg_step_advance / bg_ddpm_step_tab / bg_ddim_step_tab / bg_dpm_step_tab).  known: {slots: (values, token mask)} of
-        a completion; bg_replace_known_tab then follows the step inside the captured body.  tables: (step coefficients,
-        replacement coefficients) of this segment, required for self.dpm, whose rows depend on the whole loop; its history
-        buffer `hist` lives in the scheduler, so it carries over from one segment to the next."""
+        (bg_step_advance / bg_ddpm_step_tab / bg_ddim_step_tab / bg_dpm_step_tab), and per-sample noise from the keys at
+        the device timestep.  known: {slots: (values, token mask)} of a completion; bg_replace_known_tab then follows the
+        step inside the captured body.  tables: (step coefficients, replacement coefficients) of this segment, required for
+        self.dpm, whose rows depend on the whole loop; its history buffer `hist` lives in the scheduler, so it carries over
+        from one segment to the next."""
         dev = self.device
         lib = _ffi.lib()
         T = len(timesteps)
@@ -374,14 +375,10 @@ class Cascade:
                 _ffi.check(lib.bg_ddim_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(),
                                                 xb.data_ptr(), seed, off0, stride, _ffi.ptr(keys), n // B, t_cur.data_ptr(),
                                                 n, coef.data_ptr(), step.data_ptr(), clip, 0, st), "bg_ddim_step_tab")
-            elif keyed:
-                _ffi.check(lib.bg_ddpm_step_tab_keyed(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(),
-                                                      xb.data_ptr(), keys.data_ptr(), n // B, t_cur.data_ptr(), n,
-                                                      coef.data_ptr(), step.data_ptr(), clip, st), "bg_ddpm_step_tab_keyed")
             else:
                 _ffi.check(lib.bg_ddpm_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(),
-                                                xb.data_ptr(), seed, off0, stride, n, coef.data_ptr(), step.data_ptr(), clip,
-                                                st), "bg_ddpm_step_tab")
+                                                xb.data_ptr(), seed, off0, stride, _ffi.ptr(keys), n // B, t_cur.data_ptr(),
+                                                n, coef.data_ptr(), step.data_ptr(), clip, st), "bg_ddpm_step_tab")
             replace(st)
 
         # warm-up outside the capture (packs the weights, allocates the workspace), then rewind the state it touched
@@ -693,8 +690,8 @@ class Cascade:
         draws it at t > 0, DDIM on every step when ddim_eta > 0, DPM on every step of "sde-dpmsolver++"); default = in-kernel
         Philox
         keyed by (cfg.seed, rank, stage): reproducible from cfg.seed, independent across ranks and stages.
-        cfg.noise == "per_sample": initial and step noise come from each sample's own streams (bg_randn_keyed and the keyed
-        step kernels), so sample b's outputs depend on its seed alone; init_noise / step_noise still take precedence.
+        cfg.noise == "per_sample": initial and step noise come from each sample's own streams (bg_randn_keyed and the fused
+        steps' sample keys), so sample b's outputs depend on its seed alone; init_noise / step_noise still take precedence.
         known: a Completion (schedules "ddpm", "ddim" and "dpm"): every stage that has known tokens replaces them before its
         first step and after every step with the known values noised to the step's level, so the rest is generated
         around them; the known parts come out as given, bit for bit.  replace_noise(stage_name, k, shape) -> tensor:

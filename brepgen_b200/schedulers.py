@@ -57,8 +57,8 @@ def sample_seed(seed: int, index: int) -> int:
 
 
 def sample_keys(seeds, stage: int) -> np.ndarray:
-    """uint64 [len(seeds)]: the Philox key of each sample's noise streams in one cascade stage (bg_randn_keyed,
-    bg_ddpm_step_keyed)"""
+    """uint64 [len(seeds)]: the Philox key of each sample's noise streams in one cascade stage (bg_randn_keyed and the
+    sample_keys of the fused steps)"""
     return np.array([mix_seed(s, stage) for s in seeds], dtype=np.uint64)
 
 
@@ -165,6 +165,23 @@ class _NoiseStreams:
 
     def advance_philox(self, n: int, steps: int):
         self._philox_offset += steps * ((n + 3) // 4)
+
+    def _step_noise(self, x: torch.Tensor, draws: bool, noise: Optional[torch.Tensor] = None, generator=None):
+        """(noise, seed, offset, keys) of a fused step on x.  A step that draws noise (DDPM: sigma != 0, DDIM: eta > 0,
+        DPM-Solver++: its SDE form) takes `noise`, else a draw from `generator` (one, or a list with one per batch
+        element), else the per-sample streams of set_sample_keys, else the batch stream, whose offset it moves past the
+        step.  A step that draws none takes none of them."""
+        if not draws:
+            return None, 0, 0, None
+        if noise is None and generator is not None:
+            noise = _generator_noise(x, generator)
+        if noise is not None:
+            return noise.to(device=x.device, dtype=torch.float32).contiguous(), 0, 0, None
+        if self._sample_seeds is not None:
+            return None, 0, 0, self.sample_key_tensor(x.shape[0], x.device)
+        seed, offset, _ = self.philox_stream(x.numel())
+        self.advance_philox(x.numel(), 1)
+        return None, seed, offset, None
 
     # ---------------------------------------------------------------- known-token replacement (B-rep completion)
     def _abar_prev(self, t: int) -> torch.Tensor:
@@ -302,31 +319,14 @@ class DDPMScheduler(_NoiseStreams):
         x, eps, eps_u, dst = _step_tensors("DDPMScheduler.step", model_output, sample, model_output_uncond, noise, out)
         t = _as_int(timestep)
         sb, sa, c_x0, c_x, sigma = self.step_coefficients(t)
-        if noise is None and generator is not None and sigma != 0.0:
-            noise = _generator_noise(x, generator)
-        if noise is not None:
-            noise = noise.to(device=x.device, dtype=torch.float32).contiguous()
+        noise, seed, offset, keys = self._step_noise(x, sigma != 0.0, noise, generator)
         n = x.numel()
         clip = float(self.config.clip_sample_range) if self.config.clip_sample else 0.0
-        if self._sample_seeds is not None:
-            keys = self.sample_key_tensor(x.shape[0], x.device)
-            with torch.cuda.device(x.device):
-                _ffi.check(_ffi.lib().bg_ddpm_step_keyed(eps.data_ptr(), _ffi.ptr(eps_u), float(guidance_w), x.data_ptr(),
-                                                        dst.data_ptr(), _ffi.ptr(noise), keys.data_ptr(), n // x.shape[0],
-                                                        t, n, sb, sa, clip, c_x0, c_x, sigma, _ffi.current_stream()),
-                           "bg_ddpm_step_keyed")
-            return SchedulerOutput(dst) if return_dict else (dst,)
-        seed, offset = 0, 0
-        if noise is None and sigma != 0.0:
-            if self._philox_seed is None:
-                self._philox_seed = mix_seed(torch.initial_seed())
-            seed = self._philox_seed
-            offset = self._philox_offset
-            self._philox_offset += (n + 3) // 4
         with torch.cuda.device(x.device):
             _ffi.check(_ffi.lib().bg_ddpm_step(eps.data_ptr(), _ffi.ptr(eps_u), float(guidance_w), x.data_ptr(),
-                                              dst.data_ptr(), _ffi.ptr(noise), seed, offset, n, sb, sa, clip, c_x0, c_x,
-                                              sigma, _ffi.current_stream()), "bg_ddpm_step")
+                                              dst.data_ptr(), _ffi.ptr(noise), seed, offset, _ffi.ptr(keys),
+                                              n // x.shape[0], t, n, sb, sa, clip, c_x0, c_x, sigma,
+                                              _ffi.current_stream()), "bg_ddpm_step")
         return SchedulerOutput(dst) if return_dict else (dst,)
 
     def add_noise(self, original_samples, noise, timesteps):
@@ -427,18 +427,8 @@ class DDIMScheduler(_NoiseStreams):
                              "`generator` or `variance_noise` stays `None`.")
         x, eps, eps_u, dst = _step_tensors("DDIMScheduler.step", model_output, sample, model_output_uncond,
                                            variance_noise, out)
-        noise, seed, offset, keys = None, 0, 0, None
+        noise, seed, offset, keys = self._step_noise(x, eta > 0, variance_noise, generator)
         n = x.numel()
-        if eta > 0:
-            noise = variance_noise if variance_noise is not None else \
-                (_generator_noise(x, generator) if generator is not None else None)
-            if noise is not None:
-                noise = noise.to(device=x.device, dtype=torch.float32).contiguous()
-            elif self._sample_seeds is not None:
-                keys = self.sample_key_tensor(x.shape[0], x.device)
-            else:
-                seed, offset, _ = self.philox_stream(n)
-                self.advance_philox(n, 1)
         with torch.cuda.device(x.device):
             _ffi.check(_ffi.lib().bg_ddim_step(eps.data_ptr(), _ffi.ptr(eps_u), float(guidance_w), x.data_ptr(),
                                               dst.data_ptr(), _ffi.ptr(noise), seed, offset, _ffi.ptr(keys),
@@ -900,18 +890,8 @@ class DPMSolverMultistepScheduler(_NoiseStreams):
         order = 1 if (self.config.solver_order == 1 or self.lower_order_nums < 1 or last) else 2
         coefs = self.step_coefficients(k, order)
         t = _as_int(timestep)
-        noise, seed, offset, keys = None, 0, 0, None
+        noise, seed, offset, keys = self._step_noise(x, sde, variance_noise, generator)
         n = x.numel()
-        if sde:
-            noise = variance_noise if variance_noise is not None else \
-                (_generator_noise(x, generator) if generator is not None else None)
-            if noise is not None:
-                noise = noise.to(device=x.device, dtype=torch.float32).contiguous()
-            elif self._sample_seeds is not None:
-                keys = self.sample_key_tensor(x.shape[0], x.device)
-            else:
-                seed, offset, _ = self.philox_stream(n)
-                self.advance_philox(n, 1)
         clip = float(self.config.clip_sample_range) if self.config.clip_sample else 0.0
         with torch.cuda.device(x.device):
             _ffi.check(_ffi.lib().bg_dpm_step(eps.data_ptr(), _ffi.ptr(eps_u), float(guidance_w), x.data_ptr(),

@@ -139,42 +139,40 @@ int bg_vae_reconstruct(BgVae* enc, BgVae* dec, const float* x, int N, int hw, co
  * ------------------------------------------------------------------------------------------------------------- */
 /* eps = eps_cond if eps_uncond == NULL else eps_cond*(1+w) - eps_uncond*w            (CFG, sample.py:134)
  * x0  = clamp((x - sqrt_one_minus_abar*eps) / sqrt_abar, -clip, clip)  (clip <= 0: no clamp)
- * out = c_x0*x0 + c_x*x + sigma*noise;   noise: explicit tensor, or Philox N(0,1) from (seed, offset) if NULL & sigma>0 */
+ * out = c_x0*x0 + c_x*x + sigma*noise
+ * noise (only read when sigma != 0): the explicit tensor if not NULL; else, when sample_keys != NULL, the per-sample
+ * streams below at timestep t (domain 0), over n / per_sample samples of per_sample elements; else the batch Philox
+ * stream (seed, offset).  Keyed: per_sample <= 0 or n not a multiple of per_sample is BG_STATUS_BAD_ARG, as are NULL
+ * pointers, sqrt_abar <= 0 and t outside 32 bits; nothing is launched then.  The keyed step is bit-identical to the step
+ * fed the tensor bg_randn_keyed(..., 0, t, ...) writes. */
 int bg_ddpm_step(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
-                 const float* noise, uint64_t seed, uint64_t offset, int64_t n, float sqrt_one_minus_abar,
-                 float sqrt_abar, float clip, float c_x0, float c_x, float sigma, void* stream);
+                 const float* noise, uint64_t seed, uint64_t offset, const uint64_t* sample_keys, int64_t per_sample,
+                 int64_t t, int64_t n, float sqrt_one_minus_abar, float sqrt_abar, float clip, float c_x0, float c_x,
+                 float sigma, void* stream);
 /* The same update in table-driven form for CUDA-graph capture of a whole denoising loop (SURVEY.md 7.2 step 4): no
  * step-specific value is a kernel argument.  coef_table[k][5] = (sqrt(1-abar_t), sqrt(abar_t), c_x0, c_x, sigma) of step k
  * (device, built once per loop from the scheduler's host tables); *step (device int32) = the current step index;
- * in-kernel Philox noise with counter offset0 + k * offset_stride.  Replaces the loop body sample.py:145-153. */
+ * batch-stream counter offset0 + k * offset_stride, or, when sample_keys != NULL, the per-sample streams at the timestep
+ * *t_cur (t_cur may be NULL only without keys).  Bit-identical to bg_ddpm_step with the same coefficients and noise.
+ * Replaces the loop body sample.py:145-153. */
 int bg_ddpm_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out, uint64_t seed,
-                     uint64_t offset0, uint64_t offset_stride, int64_t n, const float* coef_table, const int32_t* step,
-                     float clip, void* stream);
+                     uint64_t offset0, uint64_t offset_stride, const uint64_t* sample_keys, int64_t per_sample,
+                     const int64_t* t_cur, int64_t n, const float* coef_table, const int32_t* step, float clip,
+                     void* stream);
 /* k = ++(*step) (clamped to n_steps - 1);  *t_cur = timesteps[k].  One tiny kernel at the top of every captured step: the
  * denoiser forward reads its timestep from t_cur (device int64), bg_ddpm_step_tab reads k. */
 int bg_step_advance(const int64_t* timesteps, int n_steps, int32_t* step, int64_t* t_cur, void* stream);
-/* Per-sample noise streams (opt-in; the functions above keep the batch-wide (seed, offset) stream).  sample_keys: device
- * uint64 [n_samples], one Philox4x32-10 key per sample.  Element j of sample b is normal (j % 4) of the block with key
+/* Per-sample noise streams (opt-in; without sample_keys the steps draw the batch-wide (seed, offset) stream).
+ * sample_keys: device uint64 [n_samples], one Philox4x32-10 key per sample.  Element j of sample b is normal (j % 4) of the block with key
  * sample_keys[b] and counter (j / 4 as 64 bits, t, domain), Box-Muller as bg_ddpm_step; a block of 4 never straddles two
  * samples.  domain 0 = DDPM step noise at timestep t, domain 1 = initial noise (t = 0), domain 2 = known-token
  * replacement noise (bg_replace_known; t = the counter word t_ctr), domain 3 = RePaint step noise (bg_repaint_step; t = the
  * list entry k), domain 4 = RePaint undo noise (bg_repaint_undo; t = k * n_trans + i).  A sample's noise is therefore a
  * function of its key alone, whatever the batch size, its position in the batch or the rank that runs it.
- * NULL sample_keys, per_sample <= 0 or n not a multiple of per_sample: BG_STATUS_BAD_ARG, nothing is launched. */
+ * bg_randn_keyed: NULL sample_keys, n_samples <= 0 or per_sample <= 0: BG_STATUS_BAD_ARG, nothing is launched. */
 /* out[b * per_sample + j] = normal j of sample b  (n_samples * per_sample fp32) */
 int bg_randn_keyed(const uint64_t* sample_keys, int64_t n_samples, int64_t per_sample, int32_t domain, int64_t t, float* out,
                    void* stream);
-/* bg_ddpm_step over n / per_sample samples of per_sample elements, noise from the per-sample streams at timestep t (domain 0)
- * unless `noise` is given.  Bit-identical to bg_ddpm_step fed the tensor bg_randn_keyed(..., 0, t, ...) writes. */
-int bg_ddpm_step_keyed(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
-                       const float* noise, const uint64_t* sample_keys, int64_t per_sample, int64_t t, int64_t n,
-                       float sqrt_one_minus_abar, float sqrt_abar, float clip, float c_x0, float c_x, float sigma,
-                       void* stream);
-/* table-driven form for graph capture: coefficients from coef_table[*step] as bg_ddpm_step_tab, timestep t from the device
- * int64 *t_cur that bg_step_advance writes; bit-identical to bg_ddpm_step_keyed at the same t. */
-int bg_ddpm_step_tab_keyed(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
-                           const uint64_t* sample_keys, int64_t per_sample, const int64_t* t_cur, int64_t n,
-                           const float* coef_table, const int32_t* step, float clip, void* stream);
 /* DDIM step (diffusers DDIMScheduler.step, prediction_type "epsilon"), fp32 in diffusers' order of operations:
  * eps   = eps_cond if eps_uncond == NULL else eps_cond*(1+w) - eps_uncond*w            (CFG, as bg_ddpm_step)
  * x0    = clamp((x - sqrt_one_minus_abar*eps) / sqrt_abar, -clip, clip)  (clip <= 0: no clamp)
@@ -182,8 +180,8 @@ int bg_ddpm_step_tab_keyed(const float* eps_cond, const float* eps_uncond, float
  * out   = sqrt_abar_prev*x0 + c_dir*e_dir + sigma*noise;   sigma = eta*sqrt((1-abar_prev)/(1-abar_t)*(1-abar_t/abar_prev)),
  *         c_dir = sqrt(1 - abar_prev - sigma^2), computed by the host scheduler.
  * noise (only read when sigma != 0): the explicit tensor if not NULL; else, when sample_keys != NULL, the per-sample
- * streams of bg_ddpm_step_keyed (domain 0, timestep t; the same normals the keyed DDPM step draws at t); else the batch
- * Philox stream (seed, offset) of bg_ddpm_step.  Keyed: per_sample <= 0 or n not a multiple of per_sample is
+ * streams at timestep t (domain 0; the same normals bg_ddpm_step draws at t); else the batch Philox stream (seed, offset)
+ * of bg_ddpm_step.  Keyed: per_sample <= 0 or n not a multiple of per_sample is
  * BG_STATUS_BAD_ARG, as are NULL pointers, sqrt_abar <= 0 and t outside 32 bits; nothing is launched then. */
 int bg_ddim_step(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
                  const float* noise, uint64_t seed, uint64_t offset, const uint64_t* sample_keys, int64_t per_sample,

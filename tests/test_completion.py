@@ -226,7 +226,7 @@ def _stage_calls(fake_lib, kind, noise, known, use_cf=False, S0=3):
     def late(t, x):
         return x.repeat(1, 2, 1) if (not use_cf and x.shape[1] == S0 and t <= 249) else x
     c._stage(cfg, torch.zeros(B, S0, 6), lambda x, t: torch.zeros_like(x), None, None, True, on_step=late, known=kn)
-    step = "bg_ddim_step" if kind == "ddim" else ("bg_ddpm_step_keyed" if noise == "per_sample" else "bg_ddpm_step")
+    step = "bg_ddim_step" if kind == "ddim" else "bg_ddpm_step"
     sched = c.ddim if kind == "ddim" else c.ddpm
     return fake_lib.named(step), fake_lib.named("bg_replace_known"), sched
 
@@ -239,7 +239,7 @@ def test_stage_counters_keys_and_untouched_step_stream(fake_lib, kind, noise):
     steps1, rep1, s1 = _stage_calls(fake_lib, kind, noise, known=True)
     assert rep0 == []
     # the step calls, their noise offsets and the scheduler's stream position are those of the run without completion
-    ptrs = (0, 1, 3, 4, 8 if kind == "ddim" else 6)      # eps, eps_uncond, x, out and sample_keys (per-run tensors)
+    ptrs = (0, 1, 3, 4, 8)      # eps, eps_uncond, x, out and sample_keys (per-run tensors)
     strip = lambda calls: [tuple(v for i, v in enumerate(a) if i not in ptrs) for a in calls]
     assert strip(steps1) == strip(steps0) and s1._philox_offset == off0
     ts = s1.timesteps.tolist()
@@ -253,7 +253,9 @@ def test_stage_counters_keys_and_untouched_step_stream(fake_lib, kind, noise):
         if kind == "ddim":
             assert all(a[8] == keys for a in steps1)                  # bg_ddim_step's sample_keys
         else:
-            assert all(a[6] == keys for a in steps1)                  # bg_ddpm_step_keyed's sample_keys
+            # bg_ddpm_step's sample_keys on every step that draws (sigma != 0), none on the last step (t = 0, sigma = 0)
+            assert [a[8] for a in steps1] == [keys] * (len(steps1) - 1) + [None]
+            assert [a[17] != 0.0 for a in steps1] == [True] * (len(steps1) - 1) + [False]
     else:
         assert all(a[R_KEYS] is None and a[R_SEED] == mix_seed(mix_seed(4, 0, 0), 2) for a in rep1)
 

@@ -128,7 +128,7 @@ def _keys(seeds, stage):
 @pytest.mark.parametrize("use_clipped", [0, 1])
 @pytest.mark.parametrize("cfg_w", [0.0, 0.6])
 @pytest.mark.parametrize("per", [7, 13, 1638])
-def test_eager_keyed_and_table_forms_agree(per, cfg_w, use_clipped):
+def test_forms_agree_and_draw_the_ddpm_step_noise(per, cfg_w, use_clipped):
     from brepgen_b200.sampler import randn_keyed
     from brepgen_b200.schedulers import DDIMScheduler, sample_seed
     f, lib, st = _lib()
@@ -182,7 +182,7 @@ def test_eager_keyed_and_table_forms_agree(per, cfg_w, use_clipped):
             z_ddpm = new()
             zero = torch.zeros_like(x)
             f.check(lib.bg_ddpm_step(zero.data_ptr(), None, 0.0, zero.data_ptr(), z_ddpm.data_ptr(), None, seed,
-                                     off0 + i * stride, n, 0.5, 1.0, 0.0, 0.0, 0.0, 1.0, st), "ddpm noise")
+                                     off0 + i * stride, None, 0, 0, n, 0.5, 1.0, 0.0, 0.0, 0.0, 1.0, st), "ddpm noise")
             torch.cuda.synchronize()
             assert torch.allclose(batch, quiet + c[4] * z_ddpm, rtol=1e-6, atol=1e-6)
 

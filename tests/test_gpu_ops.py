@@ -173,7 +173,7 @@ def test_layernorm(rows, act):
     assert rel_l2(y.float(), ref) < 1e-3
 
 
-def test_ddpm_and_pndm_step_kernels():
+def test_fused_ddpm_and_pndm_steps():
     f = _ffi()
     g = torch.Generator(device="cuda").manual_seed(3)
     n = 100003
@@ -181,7 +181,7 @@ def test_ddpm_and_pndm_step_kernels():
     out = torch.empty(n, device="cuda")
     w, sb, sa, clip, c0, cx, sig = 0.6, 0.8, 0.6, 3.0, 0.3, 0.69, 0.05
     f.check(f.lib().bg_ddpm_step(eps.data_ptr(), eps_u.data_ptr(), w, x.data_ptr(), out.data_ptr(), noise.data_ptr(), 0, 0,
-                                n, sb, sa, clip, c0, cx, sig, f.current_stream()))
+                                None, 0, 0, n, sb, sa, clip, c0, cx, sig, f.current_stream()))
     e = eps * (1 + w) - eps_u * w
     ref = c0 * ((x - sb * e) / sa).clamp(-clip, clip) + cx * x + sig * noise
     assert (out - ref).abs().max() < 1e-5
@@ -189,8 +189,8 @@ def test_ddpm_and_pndm_step_kernels():
     zeros = torch.zeros(n, device="cuda")
     o1, o2 = torch.empty(n, device="cuda"), torch.empty(n, device="cuda")
     for o in (o1, o2):
-        f.check(f.lib().bg_ddpm_step(zeros.data_ptr(), None, 0.0, zeros.data_ptr(), o.data_ptr(), None, 1234, 77, n, 0.0,
-                                    1.0, 0.0, 0.0, 0.0, 1.0, f.current_stream()))
+        f.check(f.lib().bg_ddpm_step(zeros.data_ptr(), None, 0.0, zeros.data_ptr(), o.data_ptr(), None, 1234, 77, None, 0,
+                                    0, n, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0, f.current_stream()))
     assert torch.equal(o1, o2)
     assert abs(float(o1.mean())) < 0.02 and abs(float(o1.std()) - 1) < 0.02
     es = [torch.randn(n, generator=g, device="cuda") for _ in range(4)]

@@ -1,8 +1,8 @@
-"""GPU tests of the per-sample noise mode (bg_randn_keyed, bg_ddpm_step_keyed, bg_ddpm_step_tab_keyed and
+"""GPU tests of the per-sample noise mode (bg_randn_keyed, bg_ddpm_step and bg_ddpm_step_tab with sample keys, and
 CascadeConfig(noise="per_sample")).
 
   * the generator against a numpy Philox4x32-10 of the same counters with float64 Box-Muller, and its statistics;
-  * the keyed step kernels against each other and against bg_ddpm_step fed the keyed noise, bit for bit;
+  * the keyed step forms against each other and against bg_ddpm_step fed the keyed noise, bit for bit;
   * noise that does not depend on the batch: sample b of a batch equals the same sample drawn alone, bit for bit;
   * small cascades: B = 5 equals five B = 1 runs, CFG, graph on / off, two simulated ranks, explicit sample seeds;
   * the benchmark's shape (B = 64, S0 = 50, E = 40) against B = 1 runs of three of its samples;
@@ -114,7 +114,7 @@ def _step_inputs(B, per, seed=0):
 
 @pytest.mark.parametrize("cfg_w", [0.0, 0.6])
 @pytest.mark.parametrize("per", [7, 13, 1638])
-def test_keyed_step_equals_batch_step_fed_keyed_noise_and_table_form(per, cfg_w):
+def test_ddpm_step_with_keys_equals_step_fed_keyed_noise_and_table_form(per, cfg_w):
     from brepgen_b200 import _ffi as f
     from brepgen_b200.schedulers import DDPMScheduler
     lib, st = f.lib(), f.current_stream()
@@ -130,16 +130,17 @@ def test_keyed_step_equals_batch_step_fed_keyed_noise_and_table_form(per, cfg_w)
     for i, t in enumerate(ts.tolist()):
         sb, sa, c_x0, c_x, sigma = sch.step_coefficients(t)
         keyed = torch.full_like(x, float("nan"))
-        f.check(lib.bg_ddpm_step_keyed(eps_c.data_ptr(), f.ptr(eps_u), cfg_w, x.data_ptr(), keyed.data_ptr(), None,
-                                       k.data_ptr(), per, t, B * per, sb, sa, 3.0, c_x0, c_x, sigma, st), "keyed")
+        f.check(lib.bg_ddpm_step(eps_c.data_ptr(), f.ptr(eps_u), cfg_w, x.data_ptr(), keyed.data_ptr(), None, 0, 0,
+                                 k.data_ptr(), per, t, B * per, sb, sa, 3.0, c_x0, c_x, sigma, st), "keyed")
         nz = randn_keyed(k, B, per, 0, t)
         fed = torch.full_like(x, float("nan"))
         f.check(lib.bg_ddpm_step(eps_c.data_ptr(), f.ptr(eps_u), cfg_w, x.data_ptr(), fed.data_ptr(), nz.data_ptr(), 0, 0,
-                                 B * per, sb, sa, 3.0, c_x0, c_x, sigma, st), "ddpm_step")
+                                 None, 0, 0, B * per, sb, sa, 3.0, c_x0, c_x, sigma, st), "ddpm_step")
         f.check(lib.bg_step_advance(ts_d.data_ptr(), len(ts), step.data_ptr(), t_cur.data_ptr(), st), "advance")
         tab = torch.full_like(x, float("nan"))
-        f.check(lib.bg_ddpm_step_tab_keyed(eps_c.data_ptr(), f.ptr(eps_u), cfg_w, x.data_ptr(), tab.data_ptr(), k.data_ptr(),
-                                           per, t_cur.data_ptr(), B * per, coef.data_ptr(), step.data_ptr(), 3.0, st), "tab")
+        f.check(lib.bg_ddpm_step_tab(eps_c.data_ptr(), f.ptr(eps_u), cfg_w, x.data_ptr(), tab.data_ptr(), 0, 0, 0,
+                                     k.data_ptr(), per, t_cur.data_ptr(), B * per, coef.data_ptr(), step.data_ptr(), 3.0,
+                                     st), "tab")
         torch.cuda.synchronize()
         assert torch.isfinite(keyed).all()
         assert torch.equal(keyed, fed), t
@@ -147,7 +148,7 @@ def test_keyed_step_equals_batch_step_fed_keyed_noise_and_table_form(per, cfg_w)
         if sigma != 0.0:     # the noise is really there
             quiet = torch.empty_like(x)
             f.check(lib.bg_ddpm_step(eps_c.data_ptr(), f.ptr(eps_u), cfg_w, x.data_ptr(), quiet.data_ptr(), None, 0, 0,
-                                     B * per, sb, sa, 3.0, c_x0, c_x, 0.0, st), "ddpm_step")
+                                     None, 0, 0, B * per, sb, sa, 3.0, c_x0, c_x, 0.0, st), "ddpm_step")
             torch.cuda.synchronize()
             assert not torch.equal(quiet, keyed)
 
@@ -284,7 +285,7 @@ def test_benchmark_shape_samples_equal_samples_run_alone(masks):
 
 
 # --------------------------------------------------------------------------------------------------------- errors
-def test_bad_keyed_arguments_are_rejected_and_launch_nothing():
+def test_bad_keyed_step_arguments_are_rejected_and_launch_nothing():
     from brepgen_b200 import _ffi as f
     lib, st = f.lib(), f.current_stream()
     B, per = 3, 8
@@ -295,24 +296,25 @@ def test_bad_keyed_arguments_are_rejected_and_launch_nothing():
     step = torch.zeros(1, dtype=torch.int32, device="cuda")
     t_cur = torch.zeros(1, dtype=torch.int64, device="cuda")
     n = B * per
+
+    def step_call(per_sample, t=5, sa=0.8):
+        return lib.bg_ddpm_step(eps.data_ptr(), None, 0.0, x.data_ptr(), out.data_ptr(), None, 0, 0, k.data_ptr(),
+                                per_sample, t, n, 0.5, sa, 3.0, 0.3, 0.6, 0.1, st)
+
+    def tab_call(per_sample, t_cur_ptr):
+        return lib.bg_ddpm_step_tab(eps.data_ptr(), None, 0.0, x.data_ptr(), out.data_ptr(), 0, 0, 0, k.data_ptr(),
+                                    per_sample, t_cur_ptr, n, coef.data_ptr(), step.data_ptr(), 3.0, st)
     cases = [
         ("randn NULL keys", lambda: lib.bg_randn_keyed(None, B, per, 0, 5, out.data_ptr(), st)),
         ("randn per_sample 0", lambda: lib.bg_randn_keyed(k.data_ptr(), B, 0, 0, 5, out.data_ptr(), st)),
         ("randn per_sample < 0", lambda: lib.bg_randn_keyed(k.data_ptr(), B, -4, 0, 5, out.data_ptr(), st)),
-        ("step NULL keys", lambda: lib.bg_ddpm_step_keyed(eps.data_ptr(), None, 0.0, x.data_ptr(), out.data_ptr(), None, None,
-                                                          per, 5, n, 0.5, 0.8, 3.0, 0.3, 0.6, 0.1, st)),
-        ("step per_sample 0", lambda: lib.bg_ddpm_step_keyed(eps.data_ptr(), None, 0.0, x.data_ptr(), out.data_ptr(), None,
-                                                             k.data_ptr(), 0, 5, n, 0.5, 0.8, 3.0, 0.3, 0.6, 0.1, st)),
-        ("step n % per_sample", lambda: lib.bg_ddpm_step_keyed(eps.data_ptr(), None, 0.0, x.data_ptr(), out.data_ptr(), None,
-                                                               k.data_ptr(), 5, 5, n, 0.5, 0.8, 3.0, 0.3, 0.6, 0.1, st)),
-        ("tab NULL keys", lambda: lib.bg_ddpm_step_tab_keyed(eps.data_ptr(), None, 0.0, x.data_ptr(), out.data_ptr(), None,
-                                                             per, t_cur.data_ptr(), n, coef.data_ptr(), step.data_ptr(), 3.0, st)),
-        ("tab per_sample < 0", lambda: lib.bg_ddpm_step_tab_keyed(eps.data_ptr(), None, 0.0, x.data_ptr(), out.data_ptr(),
-                                                                  k.data_ptr(), -1, t_cur.data_ptr(), n, coef.data_ptr(),
-                                                                  step.data_ptr(), 3.0, st)),
-        ("tab n % per_sample", lambda: lib.bg_ddpm_step_tab_keyed(eps.data_ptr(), None, 0.0, x.data_ptr(), out.data_ptr(),
-                                                                  k.data_ptr(), 7, t_cur.data_ptr(), n, coef.data_ptr(),
-                                                                  step.data_ptr(), 3.0, st)),
+        ("step per_sample 0", lambda: step_call(0)),
+        ("step n % per_sample", lambda: step_call(5)),
+        ("step t outside 32 bits", lambda: step_call(per, t=2 ** 32)),
+        ("step sqrt_abar 0", lambda: step_call(per, sa=0.0)),
+        ("tab per_sample < 0", lambda: tab_call(-1, t_cur.data_ptr())),
+        ("tab n % per_sample", lambda: tab_call(7, t_cur.data_ptr())),
+        ("tab keyed NULL t_cur", lambda: tab_call(per, None)),
     ]
     l0 = lib.bg_launch_count()
     for name, call in cases:

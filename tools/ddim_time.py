@@ -65,8 +65,8 @@ def step_times(B=64, per=100 * 40 * 18, iters=200, rounds=15):
     c_ddpm = ddpm.step_coefficients(500)
 
     def ddpm_fn(u):
-        return lambda: lib.bg_ddpm_step(eps_c.data_ptr(), f.ptr(u), 0.6, x.data_ptr(), out.data_ptr(), None, 7, 0, n,
-                                        *c_ddpm[:2], 3.0, *c_ddpm[2:], st)
+        return lambda: lib.bg_ddpm_step(eps_c.data_ptr(), f.ptr(u), 0.6, x.data_ptr(), out.data_ptr(), None, 7, 0, None, 0,
+                                        500, n, *c_ddpm[:2], 3.0, *c_ddpm[2:], st)
 
     def ddim_fn(u, eta):
         c = ddim.step_coefficients(500, eta)

@@ -1,6 +1,6 @@
-"""Time the per-sample-keyed DDPM step (bg_ddpm_step_keyed) against the batch-stream step (bg_ddpm_step) at the edgeZV size
-of the benchmark (B = 64 samples of 100 x 40 x 18 = 72 000 elements: 4.6 M), with and without the CFG combine.  Both draw
-their noise in the kernel.  Rounds alternate between the two kernels; prints the median per-launch time of each.
+"""Time the DDPM step (bg_ddpm_step) with per-sample keys against the step with the batch stream at the edgeZV size of the
+benchmark (B = 64 samples of 100 x 40 x 18 = 72 000 elements: 4.6 M), with and without the CFG combine.  Both draw
+their noise in the kernel.  Rounds alternate between the two forms; prints the median per-launch time of each.
     python tools/ddpm_keyed_time.py
 """
 import os
@@ -24,13 +24,9 @@ def main(B=64, per=100 * 40 * 18, iters=200, rounds=15):
     lib, st = f.lib(), f.current_stream()
     coef = (0.5, 0.8, 0.3, 0.6, 0.1)
 
-    def batch(u):
-        return lambda: lib.bg_ddpm_step(eps_c.data_ptr(), f.ptr(u), 0.6, x.data_ptr(), out.data_ptr(), None, 7, 0, n, *coef[:2],
-                                        3.0, *coef[2:], st)
-
-    def keyed(u):
-        return lambda: lib.bg_ddpm_step_keyed(eps_c.data_ptr(), f.ptr(u), 0.6, x.data_ptr(), out.data_ptr(), None,
-                                              keys.data_ptr(), per, 500, n, *coef[:2], 3.0, *coef[2:], st)
+    def step(u, k):
+        return lambda: lib.bg_ddpm_step(eps_c.data_ptr(), f.ptr(u), 0.6, x.data_ptr(), out.data_ptr(), None, 7, 0, f.ptr(k),
+                                        per, 500, n, *coef[:2], 3.0, *coef[2:], st)
 
     def timed(fn):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -41,7 +37,7 @@ def main(B=64, per=100 * 40 * 18, iters=200, rounds=15):
         torch.cuda.synchronize()
         return e0.elapsed_time(e1) * 1000.0 / iters
     for cfg, u in (("no CFG", None), ("CFG", eps_u)):
-        fb, fk = batch(u), keyed(u)
+        fb, fk = step(u, None), step(u, keys)
         assert fb() == 0 and fk() == 0
         for _ in range(3):
             timed(fb), timed(fk)
@@ -51,7 +47,7 @@ def main(B=64, per=100 * 40 * 18, iters=200, rounds=15):
             tk.append(timed(fk))
         mb, mk = statistics.median(tb), statistics.median(tk)
         nbytes = n * 4 * (4 if u is not None else 3)
-        print(f"{cfg}: n = {n}  bg_ddpm_step {mb:.1f} us ({nbytes / mb / 1e3:.0f} GB/s)  bg_ddpm_step_keyed {mk:.1f} us "
+        print(f"{cfg}: n = {n}  batch stream {mb:.1f} us ({nbytes / mb / 1e3:.0f} GB/s)  keyed {mk:.1f} us "
               f"({nbytes / mk / 1e3:.0f} GB/s)  keyed / batch = {mk / mb:.3f}  (spread {min(tb):.1f}-{max(tb):.1f} / "
               f"{min(tk):.1f}-{max(tk):.1f} us)", flush=True)
 

@@ -33,14 +33,14 @@ run("attention", T.test_attention, 1, 300, None, 0)
 run("attention", T.test_attention, 2, 257, "rand", 0)
 run("attention", T.test_attention, 2, 1000, "blocks", 1)
 run("layernorm", T.test_layernorm, 77, 0)
-run("scheduler steps", T.test_ddpm_and_pndm_step_kernels)
+run("scheduler steps", T.test_fused_ddpm_and_pndm_steps)
 import test_gpu_sample_noise as SN   # noqa: E402
 run("keyed noise", SN.test_randn_keyed_matches_numpy_philox, 13, 1, 0)
-run("keyed steps", SN.test_keyed_step_equals_batch_step_fed_keyed_noise_and_table_form, 7, 0.6)
-run("keyed bad args", SN.test_bad_keyed_arguments_are_rejected_and_launch_nothing)
+run("keyed steps", SN.test_ddpm_step_with_keys_equals_step_fed_keyed_noise_and_table_form, 7, 0.6)
+run("keyed bad args", SN.test_bad_keyed_step_arguments_are_rejected_and_launch_nothing)
 import test_gpu_ddim as DD   # noqa: E402
 run("ddim step", DD.test_step_matches_float64, 0, 10, False, 0.5)
-run("ddim forms", DD.test_eager_keyed_and_table_forms_agree, 7, 0.6, 1)
+run("ddim forms", DD.test_forms_agree_and_draw_the_ddpm_step_noise, 7, 0.6, 1)
 run("ddim bad args", DD.test_bad_arguments_are_rejected_and_launch_nothing)
 import test_gpu_dpm as DP   # noqa: E402
 run("dpm step", DP.test_step_matches_float64, 10, "sde-dpmsolver++")
