@@ -55,6 +55,7 @@ SIGNATURES = {
     "bg_dpm_step_tab": (i32, [vp, vp, f32, vp, vp, vp, u64, u64, u64, vp, i64, vp, i64, vp, vp, f32, vp]),
     "bg_replace_known": (i32, [vp, vp, vp, i64, i64, vp, u64, vp, i64, i64, f32, f32, vp]),
     "bg_replace_known_tab": (i32, [vp, vp, vp, i64, i64, u64, vp, i64, vp, vp, vp, vp]),
+    "bg_add_noise_gather": (i32, [vp, i64, vp, i64, i32, f32, f32, f32, vp, vp, i64, i32, i64, vp, vp]),
     "bg_repaint_step": (i32, [vp, vp, f32, vp, vp, vp, vp, i64, vp, u64, vp, i64, i64, i64, f32, f32, f32, f32, f32, f32,
                               f32, vp]),
     "bg_repaint_step_tab": (i32, [vp, vp, f32, vp, vp, vp, vp, i64, u64, vp, i64, i64, vp, vp, f32, vp]),
@@ -64,6 +65,8 @@ SIGNATURES = {
     "bg_axpby": (i32, [vp, f32, vp, f32, vp, i64, vp]),
     "bg_dedup_surfaces": (i32, [vp, i32, i32, f32, vp, vp, vp]),
     "bg_dedup_edges": (i32, [vp, vp, i32, i32, i32, f32, vp, vp]),
+    "bg_dedup_surfaces_index": (i32, [vp, i32, i32, f32, vp, vp, vp, vp]),
+    "bg_fill_index": (i32, [vp, vp, i64, i64, i32, i32, vp, vp]),
     "bg_edge_endpoints": (i32, [vp, vp, f32, i64, vp, vp]),
     "bg_nn_exclude": (i32, [vp, vp, vp, i32, vp, vp]),
     "bg_pairs_within": (i32, [vp, i32, f32, vp, vp]),

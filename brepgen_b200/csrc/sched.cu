@@ -69,6 +69,51 @@ __global__ void __launch_bounds__(256) randn_keyed_kernel(const RandnKeyedP p) {
   }
 }
 
+// Start of a varied stage (SDEdit: diffusers' img2img add_noise on a gathered source): for every element i of output
+// token g = i / per_token,  out[i] = sa*(scale*src[index[g] * per_token + i % per_token]) + sb*z[i],  every product and
+// the sum rounded on its own (the fp32 torch expression).  index[g] == -1: out[i] = z[i] (a slot without a source starts
+// from pure noise); any other index outside [0, n_src): NaN.  z: explicit `noise`, else the per-sample keys (keyed_normal4
+// at counter (e / 4, t, domain), e = i % per_sample: bg_randn_keyed's normals).  One thread per group of 4 elements of a
+// sample, as the keyed kernels; without keys the whole tensor is one sample.
+struct GatherP {
+  const float *src, *noise;
+  const int* index;
+  float* out;
+  long long n, per_sample, per_token, n_src;
+  float scale, sa, sb;
+  const unsigned long long* keys;
+  uint32_t t, domain;
+};
+__global__ void __launch_bounds__(256) add_noise_gather_kernel(const GatherP p) {
+  const long long gps = (p.per_sample + 3) / 4, ng = (p.n / p.per_sample) * gps;
+  for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += (long long)gridDim.x * blockDim.x) {
+    const long long b = g / gps, q = g - b * gps;
+    const long long i0 = b * p.per_sample + q * 4;
+    const int cnt = (int)min(4ll, p.per_sample - q * 4);
+    float z[4] = {0.f, 0.f, 0.f, 0.f};
+    if (p.noise) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (j < cnt) z[j] = p.noise[i0 + j];
+    } else {
+      keyed_normal4(p.keys[b], (unsigned long long)q, p.t, p.domain, z);
+    }
+    long long tok = i0 / p.per_token, r = i0 - tok * p.per_token;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if (j < cnt) {
+        const long long s = p.index[tok];
+        float o;
+        if (s == -1) o = z[j];
+        else if (s < 0 || s >= p.n_src) o = __int_as_float(0x7fc00000);
+        else o = __fadd_rn(__fmul_rn(p.sa, __fmul_rn(p.scale, p.src[s * p.per_token + r])), __fmul_rn(p.sb, z[j]));
+        p.out[i0 + j] = o;
+        if (++r == p.per_token) { ++tok; r = 0; }
+      }
+    }
+  }
+}
+
 // The four normals the DDPM, DDIM and DPM-Solver++ steps add to group q of sample b: the per-sample stream of keys[b] at
 // timestep t (domain 0) when keys != NULL, else the batch stream (seed, offset + q): the same Philox block under key seed
 // at counter (offset + q, 0, 0).  Without keys the whole tensor is one sample (per_sample = n), so q is the batch stream's
@@ -527,6 +572,27 @@ int bg_randn_keyed(const uint64_t* sample_keys, int64_t n_samples, int64_t per_s
   p.n_samples = n_samples; p.per_sample = per_sample; p.domain = (uint32_t)domain; p.t = (uint32_t)t;
   randn_keyed_kernel<<<grid_for(n_samples * ((per_sample + 3) / 4)), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
   return check_launch("randn_keyed_kernel launch");
+}
+
+int bg_add_noise_gather(const float* src, int64_t n_src_tokens, const int32_t* index, int64_t n_tokens, int32_t dim,
+                        float scale, float sqrt_abar, float sqrt_one_minus_abar, const float* noise,
+                        const uint64_t* sample_keys, int64_t tokens_per_sample, int32_t domain, int64_t t, float* out,
+                        void* stream) {
+  BG_REQUIRE(src && index && out && n_src_tokens > 0 && n_tokens > 0 && dim > 0, "add_noise_gather: bad arguments");
+  BG_REQUIRE((noise == nullptr) != (sample_keys == nullptr), "add_noise_gather: give exactly one of noise and sample_keys");
+  BG_REQUIRE(!sample_keys || (tokens_per_sample > 0 && n_tokens % tokens_per_sample == 0),
+             "add_noise_gather: n_tokens must be a positive multiple of tokens_per_sample");
+  BG_REQUIRE(domain >= 0 && t >= 0 && t <= 0xFFFFFFFFll, "add_noise_gather: domain and t must be 32-bit unsigned values");
+  GatherP p = {};
+  p.src = src; p.noise = noise; p.index = index; p.out = out;
+  p.n = n_tokens * dim; p.per_token = dim; p.n_src = n_src_tokens;
+  p.scale = scale; p.sa = sqrt_abar; p.sb = sqrt_one_minus_abar;
+  p.keys = reinterpret_cast<const unsigned long long*>(sample_keys);
+  p.per_sample = sample_keys ? tokens_per_sample * dim : p.n;
+  p.t = (uint32_t)t; p.domain = (uint32_t)domain;
+  add_noise_gather_kernel<<<grid_for((p.n / p.per_sample) * ((p.per_sample + 3) / 4)), 256, 0,
+                            reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch("add_noise_gather_kernel launch");
 }
 
 int bg_ddim_step(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,

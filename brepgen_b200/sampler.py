@@ -10,6 +10,8 @@ reshapes (sample.py:284-294).  Differences, all result-preserving:
     (few-step sampling of the same DDPM-trained denoisers), "dpm" = N DPM-Solver++ steps for every stage (the
     second-order multistep sampler of the same denoisers) and "repaint" = diffusers' RePaint list of DDIM-form steps and
     undo steps per stage (resampling, for completion).
+Beyond the reference: completion (known=Completion) and variations (source=Variation: SDEdit, each stage re-noised to a
+chosen strength and denoised again, or kept as given).
 Everything past sample.py:299 (OpenCASCADE post-processing) is out of scope (SURVEY.md section 2).
 
 Batch sharding across GPUs: samples are independent through every stage, so each rank runs its own shard and there is
@@ -18,13 +20,13 @@ no collective on the hot path; `gather_outputs` is the one optional all_gather a
 from __future__ import annotations
 
 from dataclasses import dataclass, replace
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import torch
 
 from . import _ffi
 from .schedulers import (DPM_ALGORITHMS, DDIMScheduler, DDPMScheduler, DPMSolverMultistepScheduler, PNDMScheduler,
-                         RePaintScheduler, repaint_entries, sample_keys, sample_seed)
+                         RePaintScheduler, dpm_timesteps, repaint_entries, sample_keys, sample_seed, strength_timesteps)
 
 NOISE_MODES = ("batch", "per_sample")
 
@@ -247,6 +249,102 @@ def check_completion(cfg: CascadeConfig, known: Completion) -> torch.Tensor:
     return n
 
 
+STAGES = ("surfPos", "surfZ", "edgePos", "edgeZV")
+
+
+@dataclass
+class Variation:
+    """A B-rep to vary with Cascade.run(source=...) (SDEdit, diffusers' img2img `strength`): each varied stage starts from
+    its source noised to an intermediate timestep and runs only the rest of the schedule.  Tensors in the units and shapes
+    Cascade.run returns for the cfg (boxes divided by 3): surfPos (B, S, 6), surfMask (B, S) bool, surfZ (B, S, 48),
+    edgePos (B, S, E, 6), edgeM (B, S, E) bool, edge_z (B, S, E, 12), edgeV (B, S, E, 6); S = 2 * num_surfaces without
+    CFG, num_surfaces with it; E = num_edges.  strength: one value in [0, 1] for all stages, or four for (surfPos, surfZ,
+    edgePos, edgeZV).  1 = a fresh sample, 0 = keep the stage as given (zero strengths must come first: a later stage is
+    conditioned on the earlier ones)."""
+    surfPos: torch.Tensor
+    surfMask: torch.Tensor
+    surfZ: torch.Tensor
+    edgePos: torch.Tensor
+    edgeM: torch.Tensor
+    edge_z: torch.Tensor
+    edgeV: torch.Tensor
+    strength: Union[float, Sequence[float]] = 1.0
+
+    @staticmethod
+    def from_outputs(out: Dict[str, torch.Tensor], strength: Union[float, Sequence[float]]) -> "Variation":
+        """a variation of an earlier Cascade.run output: run(cfg, source=Variation.from_outputs(out, 0.5))"""
+        return Variation(*(out[k] for k in ("surfPos", "surfMask", "surfZ", "edgePos", "edgeM", "edge_z", "edgeV")),
+                         strength=strength)
+
+
+def stage_timesteps(cfg: CascadeConfig) -> torch.Tensor:
+    """the timestep list every stage of cfg's "ddpm", "ddim" or "dpm" schedule runs (as Cascade.run sets it)"""
+    if cfg.schedule == "dpm":
+        return torch.from_numpy(dpm_timesteps(1000, int(cfg.dpm_steps), "linspace"))
+    s = DDIMScheduler() if cfg.schedule == "ddim" else DDPMScheduler()
+    s.set_timesteps(int(cfg.ddim_steps if cfg.schedule == "ddim" else cfg.ddpm_steps))
+    return s.timesteps
+
+
+def start_slots(cfg: CascadeConfig, t0: int) -> int:
+    """face slots of a plain run at timestep t0: num_surfaces before the late increase of a non-CFG run (t > 249), else S"""
+    S = cfg.num_surfaces if cfg.use_cf else 2 * cfg.num_surfaces
+    return cfg.num_surfaces if (not cfg.use_cf and t0 > 249) else S
+
+
+def check_variation(cfg: CascadeConfig, source: Variation) -> Tuple[float, float, float, float]:
+    """raises on a Variation `cfg` cannot run (host checks only: nothing is launched); returns the four stage strengths"""
+    if cfg.schedule not in ("ddpm", "ddim", "dpm"):
+        raise NotImplementedError(f"variations need schedule 'ddpm', 'ddim' or 'dpm', got {cfg.schedule!r}: the "
+                                  "'reference' hybrid starts with PNDM's Runge-Kutta warm-up, and 'repaint' is for completion")
+    if cfg.dense_masks or cfg.ragged_masks:
+        raise ValueError("variations run the de-duplication; dense_masks and ragged_masks are benchmark modes")
+    B, E = cfg.batch_size, cfg.num_edges
+    S = cfg.num_surfaces if cfg.use_cf else 2 * cfg.num_surfaces
+    want = {"surfPos": (B, S, 6), "surfMask": (B, S), "surfZ": (B, S, 48), "edgePos": (B, S, E, 6), "edgeM": (B, S, E),
+            "edge_z": (B, S, E, 12), "edgeV": (B, S, E, 6)}
+    for name, shape in want.items():
+        t = getattr(source, name)
+        if not torch.is_tensor(t) or tuple(t.shape) != shape:
+            raise ValueError(f"Variation.{name} must be a tensor of shape {shape}, got "
+                             f"{tuple(t.shape) if torch.is_tensor(t) else type(t).__name__}")
+        if name in ("surfMask", "edgeM"):
+            if t.dtype != torch.bool:
+                raise ValueError(f"Variation.{name} must be a bool tensor (True = padded)")
+        elif not t.dtype.is_floating_point:
+            raise ValueError(f"Variation.{name} must be a floating-point tensor, got {t.dtype}")
+    st = source.strength
+    st = [st] * 4 if isinstance(st, (int, float)) else list(st)
+    if len(st) != 4:
+        raise ValueError(f"Variation.strength must be one value or four (surfPos, surfZ, edgePos, edgeZV), got {len(st)}")
+    st = [float(v) for v in st]
+    ts = stage_timesteps(cfg)
+    for name, v in zip(STAGES, st):
+        try:
+            strength_timesteps(ts, v)
+        except ValueError as e:
+            raise ValueError(f"Variation strength of {name}: {e}") from None
+    first = next((i for i, v in enumerate(st) if v > 0), 4)
+    if any(v == 0 for v in st[first:]):
+        raise ValueError(f"Variation strengths {st}: zero strengths must come first (a stage is conditioned on the ones "
+                         "before it, so it cannot be kept while they change)")
+    mask = source.surfMask.cpu()
+    if bool((source.edgeM[..., 0].cpu() & ~mask).any()):
+        raise ValueError("Variation.edgeM[..., 0] is set on a valid face: edge slot 0 of a face is always valid")
+    if st[0] > 0:
+        t0 = int(strength_timesteps(ts, st[0])[0])
+        slots = start_slots(cfg, t0)
+        nv = (~mask).sum(1)
+        if bool((nv > slots).any()):
+            lim = max((v for v in ts.tolist() if v <= 249), default=None)
+            k = len(ts) - ts.tolist().index(lim) if lim is not None else None
+            hint = f"; a surfPos strength below {(k + 1) / len(ts):g} starts at t <= 249 with {S} slots" if k else ""
+            raise ValueError(f"Variation: samples {torch.nonzero(nv > slots).flatten().tolist()} have more valid faces "
+                             f"({nv.max().item()}) than the {slots} face slots a run has at t = {t0}, where a surfPos "
+                             f"strength of {st[0]} starts{hint}")
+    return tuple(st)
+
+
 def randn_keyed(seeds: Sequence[int], stage: int, shape, device, domain: int = 1, t: int = 0) -> torch.Tensor:
     """(len(seeds), *shape[1:]) fp32 normals from the per-sample streams (bg_randn_keyed); default domain 1 = initial noise"""
     B = len(seeds)
@@ -268,6 +366,35 @@ def dedup_surfaces(surfPos: torch.Tensor, threshold: float):
         _ffi.check(_ffi.lib().bg_dedup_surfaces(x.data_ptr(), B, S, float(threshold), out.data_ptr(), mask.data_ptr(),
                                                _ffi.current_stream()), "bg_dedup_surfaces")
     return out, mask
+
+
+def dedup_surfaces_index(surfPos: torch.Tensor, threshold: float):
+    """dedup_surfaces plus the input slot of every survivor (B, S) int32, -1 past them"""
+    B, S, _ = surfPos.shape
+    x = surfPos.float().contiguous()
+    out = torch.empty_like(x)
+    mask = torch.empty(B, S, dtype=torch.bool, device=x.device)
+    idx = torch.empty(B, S, dtype=torch.int32, device=x.device)
+    with torch.cuda.device(x.device):
+        _ffi.check(_ffi.lib().bg_dedup_surfaces_index(x.data_ptr(), B, S, float(threshold), out.data_ptr(),
+                                                     mask.data_ptr(), idx.data_ptr(), _ffi.current_stream()),
+                   "bg_dedup_surfaces_index")
+    return out, mask, idx
+
+
+def fill_index(src_mask: torch.Tensor, out_slots: int, row_map: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """pad_repeat gather map (bg_fill_index): src_mask (..., in_slots) bool, True = padded; row_map (rows,) int32 source
+    row of each output row (-1 = none), default the identity.  Returns (rows, out_slots) int32 flat source-token indices."""
+    m = src_mask.to(torch.uint8).contiguous()
+    in_slots = m.shape[-1]
+    n_src = m.numel() // in_slots
+    rows = n_src if row_map is None else row_map.numel()
+    rm = None if row_map is None else row_map.to(torch.int32).contiguous()
+    out = torch.empty(rows, out_slots, dtype=torch.int32, device=m.device)
+    with torch.cuda.device(m.device):
+        _ffi.check(_ffi.lib().bg_fill_index(m.data_ptr(), _ffi.ptr(rm), rows, n_src, in_slots, out_slots, out.data_ptr(),
+                                           _ffi.current_stream()), "bg_fill_index")
+    return out
 
 
 def dedup_edges(edgePos: torch.Tensor, surfMask: torch.Tensor, threshold: float):
@@ -435,8 +562,9 @@ class Cascade:
                     hi = len(ts_list)
                 tabs = None
                 if isinstance(sched, DPMSolverMultistepScheduler):
-                    # a segment after the late increase restarts the solver (first order); rows depend on the whole loop
-                    tabs = (sched.coefficient_table(timesteps, restart=lo if lo else None)[lo:hi],
+                    # each segment starts the solver (first order): the loop's first step, a variation's truncated list
+                    # starting mid-table, and a segment after the late increase; rows depend on the whole loop
+                    tabs = (sched.coefficient_table(timesteps, restart=lo)[lo:hi],
                             sched.replace_table(timesteps)[lo:hi])
                 x = self._loop_graph(cfg, sched, timesteps[lo:hi], x, fwd, known, tabs)
                 lo = hi
@@ -604,7 +732,9 @@ class Cascade:
     _STAGE_ID = {"surfPos": 0, "surfZ": 1, "edgePos": 2, "edgeZV": 3}
 
     def _stage(self, cfg, x, fwd, label2, gen, hybrid_ddpm_tail: bool, on_step=None, noise_fn=None, name="surfPos",
-               known=None, rnoise_fn=None, unoise_fn=None):
+               known=None, rnoise_fn=None, unoise_fn=None, timesteps=None):
+        """one stage's denoising loop from x; timesteps: a tail of the schedule's list to run instead of all of it (a
+        variation; schedules "ddpm", "ddim" and "dpm")"""
         seeds = getattr(self, "_sample_seeds", None)
         if cfg.schedule == "dpm" and (self.dpm.config.solver_order, self.dpm.config.algorithm_type) != \
                 (cfg.dpm_order, cfg.dpm_algorithm):
@@ -616,17 +746,20 @@ class Cascade:
             noisy.set_noise_seed(*getattr(self, "_noise_key", (int(cfg.seed), 0)), self._STAGE_ID[name])
         if cfg.schedule == "ddim":
             self.ddim.set_timesteps(cfg.ddim_steps)
-            return self._loop(cfg, self.ddim, self.ddim.timesteps, x, fwd, label2, gen, on_step, noise_fn, known, rnoise_fn)
+            ts = self.ddim.timesteps if timesteps is None else timesteps
+            return self._loop(cfg, self.ddim, ts, x, fwd, label2, gen, on_step, noise_fn, known, rnoise_fn)
         if cfg.schedule == "dpm":
             self.dpm.set_timesteps(cfg.dpm_steps)
-            return self._loop(cfg, self.dpm, self.dpm.timesteps, x, fwd, label2, gen, on_step, noise_fn, known, rnoise_fn)
+            ts = self.dpm.timesteps if timesteps is None else timesteps
+            return self._loop(cfg, self.dpm, ts, x, fwd, label2, gen, on_step, noise_fn, known, rnoise_fn)
         if cfg.schedule == "repaint":
             self.repaint.eta = float(cfg.repaint_eta)
             self.repaint.set_timesteps(cfg.repaint_steps, cfg.repaint_jump_length, cfg.repaint_jump_n_sample)
             return self._loop_repaint(cfg, self.repaint, x, fwd, on_step, noise_fn, known, unoise_fn)
         if cfg.schedule == "ddpm":
             self.ddpm.set_timesteps(cfg.ddpm_steps)
-            return self._loop(cfg, self.ddpm, self.ddpm.timesteps, x, fwd, label2, gen, on_step, noise_fn, known, rnoise_fn)
+            ts = self.ddpm.timesteps if timesteps is None else timesteps
+            return self._loop(cfg, self.ddpm, ts, x, fwd, label2, gen, on_step, noise_fn, known, rnoise_fn)
         # the shipped hybrid: PNDM(200) then, for the position stages, DDPM(1000)[-250:]
         self.pndm.set_timesteps(200)
         ts = self.pndm.timesteps[:158] if hybrid_ddpm_tail else self.pndm.timesteps
@@ -682,10 +815,37 @@ class Cascade:
                              edgeV=pad(f32(known.edgeV), S))
         return kn
 
+    # ------------------------------------------------------------------ variations
+    def _vary_start(self, name, shape, src, index, scale, t0, init_noise, seeds, cpu_gen):
+        """the start of a varied stage (bg_add_noise_gather): sa*(scale*src[index]) + sb*z with (sa, sb) of add_noise at
+        t0; index (int32, one per token of `shape`) into the tokens of src, -1 = pure noise.  z: init_noise[name], else the
+        per-sample keys of the stage drawn in the kernel (bg_randn_keyed's initial noise), else the CPU generator."""
+        dev = self.device
+        dim = shape[-1]
+        out = torch.empty(shape, dtype=torch.float32, device=dev)
+        n_tok = out.numel() // dim
+        z = keys = None
+        if init_noise is not None and name in init_noise:
+            z = init_noise[name].to(device=dev, dtype=torch.float32).contiguous()
+            if tuple(z.shape) != tuple(shape):
+                raise ValueError(f"init_noise[{name!r}] has shape {tuple(z.shape)}; this variation starts at {tuple(shape)}")
+        elif seeds is not None:
+            keys = torch.from_numpy(sample_keys(seeds, self._STAGE_ID[name]).view("int64")).to(dev)
+        else:
+            z = torch.randn(shape, generator=cpu_gen).to(dev)
+        sa, sb = self.ddpm.replace_coefficients(t0, initial=True)
+        src = src.reshape(-1, dim)
+        idx = index.to(torch.int32).contiguous()
+        with torch.cuda.device(dev):
+            _ffi.check(_ffi.lib().bg_add_noise_gather(src.data_ptr(), src.shape[0], idx.data_ptr(), n_tok, dim,
+                                                     float(scale), sa, sb, _ffi.ptr(z), _ffi.ptr(keys), n_tok // shape[0],
+                                                     1, 0, out.data_ptr(), _ffi.current_stream()), "bg_add_noise_gather")
+        return out
+
     # ------------------------------------------------------------------ the cascade
     @torch.no_grad()
     def run(self, cfg: CascadeConfig, init_noise: Optional[Dict[str, torch.Tensor]] = None, step_noise=None,
-            known: Optional[Completion] = None, replace_noise=None, undo_noise=None):
+            known: Optional[Completion] = None, replace_noise=None, undo_noise=None, source: Optional[Variation] = None):
         """step_noise(stage_name, k, shape) -> tensor: explicit DDPM / DDIM / DPM step noise of step k (parity runs; DDPM
         draws it at t > 0, DDIM on every step when ddim_eta > 0, DPM on every step of "sde-dpmsolver++"); default = in-kernel
         Philox
@@ -696,12 +856,21 @@ class Cascade:
         first step and after every step with the known values noised to the step's level, so the rest is generated
         around them; the known parts come out as given, bit for bit.  replace_noise(stage_name, k, shape) -> tensor:
         explicit noise of that replacement (k = -1 before the first step; parity runs), mirroring step_noise.
+        source: a Variation (schedules "ddpm", "ddim" and "dpm"; not with known): each stage with strength s > 0 starts
+        from its source noised to the first timestep of strength_timesteps(list, s) and runs that tail of the list; a
+        stage with strength 0 is not run and returns the source as given, bit for bit.  A varied stage's slots take
+        their source tokens in the trainers' pad_repeat layout (bg_fill_index), across the face de-duplication
+        (bg_dedup_surfaces_index); slots without a source start from pure noise.  init_noise[name] is the start noise z
+        of a varied stage (shape: the stage's starting shape).
         schedule "repaint": step_noise(stage_name, k, shape) is the one z of the step at list entry k (drawn at every
         step); undo_noise(stage_name, k, (n, *shape)) the normals of the undo step at entry k.  Known tokens are kept by
         the RePaint step itself (no separate replacement: replace_noise is not used), and known=None is DDIM with
         resampling."""
         check_schedule(cfg)
+        if source is not None and known is not None:
+            raise ValueError("Cascade.run: a variation (source=) cannot be combined with a completion (known=)")
         n_known = check_completion(cfg, known) if known is not None else None
+        strength = check_variation(cfg, source) if source is not None else None
         seeds = per_sample_seeds(cfg)
         self._sample_seeds = seeds
         dev = self.device
@@ -744,56 +913,94 @@ class Cascade:
                 return x.repeat(1, 2, 1)
             return x
 
-        surfPos = noise("surfPos", (B, S0, 6))
-        surfPos = self._stage(cfg, surfPos, lambda x, t: self.m["surfpos"](x, t, label2), label2, gen, True,
-                              on_step=late_increase, noise_fn=nf("surfPos"), name="surfPos", known=kn.get("surfPos"),
-                              rnoise_fn=rnf("surfPos"),
-                              unoise_fn=unf("surfPos"))
-        if not cfg.use_cf and surfPos.shape[1] == S0:
-            surfPos = surfPos.repeat(1, 2, 1)
+        # a variation: the source on the device, the tail of the list each varied stage runs (None: kept), and where the
+        # start of each varied stage takes its tokens from (flat source-token indices, -1 = none)
+        var = source is not None
+        tails, src = {}, {}
+        if var:
+            full = stage_timesteps(cfg)
+            tails = {name: strength_timesteps(full, v) if v > 0 else None for name, v in zip(STAGES, strength)}
+            for k in ("surfPos", "surfZ", "edgePos", "edge_z", "edgeV", "surfMask", "edgeM"):
+                t = getattr(source, k)
+                src[k] = t.to(device=dev, dtype=t.dtype if t.dtype == torch.bool else torch.float32, copy=True).contiguous()
+            src["edgeZV"] = torch.cat([src["edge_z"], src["edgeV"]], -1)
+        kept = lambda name: var and tails[name] is None
 
-        # STEP 1-2 duplicate faces (sample.py:159-183)
+        def vary(name, shape, index, scale):
+            return self._vary_start(name, shape, src[name], index, scale, int(tails[name][0]), init_noise, seeds, cpu_gen)
+
         mask_gen = torch.Generator().manual_seed(cfg.seed + 12345)
-        if cfg.ragged_masks:
-            nv = torch.randint(max(1, S // 8), max(2, S // 2) + 1, (B,), generator=mask_gen)
-            surfMask = (torch.arange(S)[None, :] >= nv[:, None]).to(dev)
-        elif cfg.dense_masks:
-            surfMask = torch.zeros(B, S, dtype=torch.bool, device=dev)
+        if kept("surfPos"):
+            surfPos, surfMask = src["surfPos"] * 3.0, src["surfMask"]
+            rows = torch.where(surfMask, -1, torch.arange(B * S, dtype=torch.int32, device=dev).view(B, S))
         else:
-            surfPos, surfMask = dedup_surfaces(surfPos, cfg.bbox_threshold)
+            if var:       # the source's valid faces repeated to the slots a plain run has at the first timestep
+                S1 = start_slots(cfg, int(tails["surfPos"][0]))
+                fill = fill_index(src["surfMask"], S1)
+            surfPos = vary("surfPos", (B, S1, 6), fill, 3.0) if var else noise("surfPos", (B, S0, 6))
+            surfPos = self._stage(cfg, surfPos, lambda x, t: self.m["surfpos"](x, t, label2), label2, gen, True,
+                                  on_step=late_increase, noise_fn=nf("surfPos"), name="surfPos", known=kn.get("surfPos"),
+                                  rnoise_fn=rnf("surfPos"), unoise_fn=unf("surfPos"), timesteps=tails.get("surfPos"))
+            if not cfg.use_cf and surfPos.shape[1] == S0:
+                surfPos = surfPos.repeat(1, 2, 1)
+
+            # STEP 1-2 duplicate faces (sample.py:159-183)
+            if cfg.ragged_masks:
+                nv = torch.randint(max(1, S // 8), max(2, S // 2) + 1, (B,), generator=mask_gen)
+                surfMask = (torch.arange(S)[None, :] >= nv[:, None]).to(dev)
+            elif cfg.dense_masks:
+                surfMask = torch.zeros(B, S, dtype=torch.bool, device=dev)
+            elif var:     # survivor k came from slot idx[k], which the late increase's repeat took from fill slot idx % S1
+                surfPos, surfMask, idx = dedup_surfaces_index(surfPos, cfg.bbox_threshold)
+                i = idx.long()
+                rows = torch.where(i >= 0, fill.gather(1, i.clamp(min=0) % S1), -1)
+            else:
+                surfPos, surfMask = dedup_surfaces(surfPos, cfg.bbox_threshold)
         sP, sM = rep2(surfPos), rep2(surfMask)
 
         # STEP 1-3 surface latents (sample.py:189-202)
-        surfZ = noise("surfZ", (B, S, 48))
-        surfZ = self._stage(cfg, surfZ, lambda x, t: self.m["surfz"](x, t, sP, sM, label2), label2, gen, False,
-                            noise_fn=nf("surfZ"), name="surfZ", known=kn.get("surfZ"), rnoise_fn=rnf("surfZ"),
-                            unoise_fn=unf("surfZ"))
+        if kept("surfZ"):
+            surfZ = src["surfZ"]
+        else:
+            surfZ = vary("surfZ", (B, S, 48), rows, 1.0) if var else noise("surfZ", (B, S, 48))
+            surfZ = self._stage(cfg, surfZ, lambda x, t: self.m["surfz"](x, t, sP, sM, label2), label2, gen, False,
+                                noise_fn=nf("surfZ"), name="surfZ", known=kn.get("surfZ"), rnoise_fn=rnf("surfZ"),
+                                unoise_fn=unf("surfZ"), timesteps=tails.get("surfZ"))
         sZ = rep2(surfZ)
 
         # STEP 2-1 edge positions (sample.py:208-236)
-        edgePos = noise("edgePos", (B, S, E, 6))
-        edgePos = self._stage(cfg, edgePos, lambda x, t: self.m["edgepos"](x, t, sP, sZ, sM, label2), label2, gen, True,
-                              noise_fn=nf("edgePos"), name="edgePos", known=kn.get("edgePos"), rnoise_fn=rnf("edgePos"),
-                              unoise_fn=unf("edgePos"))
-
-        # STEP 2-2 duplicate edges per face (sample.py:242-261)
-        if cfg.ragged_masks:
-            ne = torch.randint(min(3, E), max(min(3, E), E // 3) + 1, (B, S), generator=mask_gen)
-            edgeM = (torch.arange(E)[None, None, :] >= ne[..., None]).to(dev) | surfMask[..., None]
-        elif cfg.dense_masks:
-            edgeM = torch.zeros(B, S, E, dtype=torch.bool, device=dev)
+        if kept("edgePos"):
+            edgePos, edgeM = src["edgePos"] * 3.0, src["edgeM"]
+            edges = torch.arange(B * S * E, dtype=torch.int32, device=dev).view(B, S, E)
         else:
-            edgeM = dedup_edges(edgePos, surfMask, cfg.bbox_threshold)
+            if var:       # the valid edges of each face's source face, repeated to E slots
+                edges = fill_index(src["edgeM"], E, rows.flatten()).view(B, S, E)
+            edgePos = vary("edgePos", (B, S, E, 6), edges, 3.0) if var else noise("edgePos", (B, S, E, 6))
+            edgePos = self._stage(cfg, edgePos, lambda x, t: self.m["edgepos"](x, t, sP, sZ, sM, label2), label2, gen,
+                                  True, noise_fn=nf("edgePos"), name="edgePos", known=kn.get("edgePos"),
+                                  rnoise_fn=rnf("edgePos"), unoise_fn=unf("edgePos"), timesteps=tails.get("edgePos"))
+
+            # STEP 2-2 duplicate edges per face (sample.py:242-261)
+            if cfg.ragged_masks:
+                ne = torch.randint(min(3, E), max(min(3, E), E // 3) + 1, (B, S), generator=mask_gen)
+                edgeM = (torch.arange(E)[None, None, :] >= ne[..., None]).to(dev) | surfMask[..., None]
+            elif cfg.dense_masks:
+                edgeM = torch.zeros(B, S, E, dtype=torch.bool, device=dev)
+            else:
+                edgeM = dedup_edges(edgePos, surfMask, cfg.bbox_threshold)
         if "edgeM" in kn:             # the known faces keep their given edge masks
             edgeM = torch.where(kn["face"][..., None], kn["edgeM"], edgeM)
         eP, eM = rep2(edgePos), rep2(edgeM)
 
         # STEP 2-3 edge latents + vertices (sample.py:267-286)
-        edgeZV = noise("edgeZV", (B, S, E, 18))
-        edgeZV = self._stage(cfg, edgeZV, lambda x, t: self.m["edgez"](x, t, eP, sP, sZ, eM, label2), label2, gen, False,
-                             noise_fn=nf("edgeZV"), name="edgeZV", known=kn.get("edgeZV"), rnoise_fn=rnf("edgeZV"),
-                             unoise_fn=unf("edgeZV"))
-        edgeZV = edgeZV.masked_fill(edgeM.unsqueeze(-1), 0.0)
+        if kept("edgeZV"):
+            edgeZV = src["edgeZV"]
+        else:
+            edgeZV = vary("edgeZV", (B, S, E, 18), edges, 1.0) if var else noise("edgeZV", (B, S, E, 18))
+            edgeZV = self._stage(cfg, edgeZV, lambda x, t: self.m["edgez"](x, t, eP, sP, sZ, eM, label2), label2, gen,
+                                 False, noise_fn=nf("edgeZV"), name="edgeZV", known=kn.get("edgeZV"),
+                                 rnoise_fn=rnf("edgeZV"), unoise_fn=unf("edgeZV"), timesteps=tails.get("edgeZV"))
+            edgeZV = edgeZV.masked_fill(edgeM.unsqueeze(-1), 0.0)
         edge_z, edgeV = edgeZV[..., :12], edgeZV[..., 12:]
 
         out = {"surfPos": surfPos / 3.0, "surfMask": surfMask, "surfZ": surfZ, "edgePos": edgePos / 3.0, "edgeM": edgeM,
@@ -802,6 +1009,13 @@ class Cascade:
             for k, v in kn["out"].items():
                 f = kn["face"].reshape(kn["face"].shape + (1,) * (v.dim() - 2))
                 out[k] = torch.where(f, v, out[k]).contiguous()
+            surfZ, edge_z = out["surfZ"], out["edge_z"]
+        if var:                       # kept stages return the source as given (the decoders see it too)
+            fields = {"surfPos": ("surfPos", "surfMask"), "surfZ": ("surfZ",), "edgePos": ("edgePos", "edgeM"),
+                      "edgeZV": ("edge_z", "edgeV")}
+            for name in STAGES:
+                if kept(name):
+                    out.update({k: src[k] for k in fields[name]})
             surfZ, edge_z = out["surfZ"], out["edge_z"]
         # decoders (sample.py:289-294)
         if cfg.decode and self.surf_vae is not None:

@@ -444,6 +444,22 @@ class DDIMScheduler(_NoiseStreams):
         return self.config.num_train_timesteps
 
 
+def strength_timesteps(timesteps, strength: float):
+    """The tail of a denoising loop that a variation at `strength` runs (diffusers' img2img get_timesteps):
+    timesteps[N - min(int(N * strength), N):], N = len(timesteps).  strength 1 is the whole loop, 0 none of it.  The sample
+    starts at add_noise(source, z, list[0]).  ValueError, as diffusers raises it: strength outside [0, 1], or a strength
+    > 0 that leaves no step (int(N * strength) == 0)."""
+    n = len(timesteps)
+    s = float(strength)
+    if not 0.0 <= s <= 1.0:
+        raise ValueError(f"The value of strength should be in [0.0, 1.0] but is {strength}")
+    k = min(int(n * s), n)
+    if s > 0 and k < 1:
+        raise ValueError(f"strength {strength} of a {n}-step schedule leaves no step (int({n} * strength) = 0); use a "
+                         f"strength of at least {1.0 / n:g}")
+    return timesteps[n - k:]
+
+
 def repaint_timesteps(num_inference_steps: int, jump_length: int, jump_n_sample: int,
                       num_train_timesteps: int = 1000) -> np.ndarray:
     """int64 timesteps of diffusers' RePaintScheduler.set_timesteps: N - 1 .. 0 in steps of one, with a jump back up by

@@ -239,6 +239,21 @@ int bg_replace_known(float* x, const float* known, const uint8_t* token_mask, in
 int bg_replace_known_tab(float* x, const float* known, const uint8_t* token_mask, int64_t n, int64_t per_token,
                          uint64_t seed, const uint64_t* sample_keys, int64_t per_sample, const int64_t* t_cur,
                          const float* coef_table, const int32_t* step, void* stream);
+/* Start of a varied stage (B-rep variations, SDEdit: diffusers' img2img add_noise on a gathered, scaled source).  out holds
+ * n_tokens tokens of dim fp32 values; for every element i of output token g = i / dim:
+ *   out[i] = sqrt_abar*(scale*src[index[g] * dim + i % dim]) + sqrt_one_minus_abar*z[i]
+ * every product and the sum rounded on its own (__fmul_rn / __fadd_rn: the fp32 torch expression of add_noise on the
+ * gathered tensor, bit for bit).  index (int32, one per output token) holds flat source-token indices into src
+ * (n_src_tokens tokens of dim values); index == -1: out = z (no source, pure noise); any other index outside
+ * [0, n_src_tokens): the token is NaN.  z: the explicit `noise` tensor, or, when sample_keys != NULL, normal (e % 4) of
+ * the per-sample stream of sample b = g / tokens_per_sample at counter (e / 4, t, domain), e = the element's index within
+ * its sample (bg_randn_keyed's normals).  Exactly one of noise and sample_keys.  BG_STATUS_BAD_ARG, launching nothing:
+ * NULL src / index / out, n_src_tokens, n_tokens or dim <= 0, both or neither noise source, (keyed) tokens_per_sample not
+ * a positive divisor of n_tokens, domain or t outside 32 bits. */
+int bg_add_noise_gather(const float* src, int64_t n_src_tokens, const int32_t* index, int64_t n_tokens, int32_t dim,
+                        float scale, float sqrt_abar, float sqrt_one_minus_abar, const float* noise,
+                        const uint64_t* sample_keys, int64_t tokens_per_sample, int32_t domain, int64_t t, float* out,
+                        void* stream);
 /* RePaint step (diffusers RePaintScheduler.step, prediction_type "epsilon"; inpainting with resampling).  Every element
  * of a token whose token_mask byte is zero gets the bg_ddim_step update, written with its expressions (bit-identical to
  * bg_ddim_step with use_clipped_eps = 0 for the same noise):
@@ -293,6 +308,20 @@ int bg_dedup_surfaces(const float* surfPos, int B, int S, float threshold, float
 /* edgePos (B,S,E,6), surf_mask (B,S) -> edge_mask (B,S,E): 1 = padded face or duplicate edge; slot 0 of a valid face = 0 */
 int bg_dedup_edges(const float* edgePos, const uint8_t* surf_mask, int B, int S, int E, float threshold,
                    uint8_t* edge_mask, void* stream);
+/* bg_dedup_surfaces plus out_index (B,S): the input slot of each survivor, -1 past them (positions and mask are those of
+ * bg_dedup_surfaces, bit for bit).  NULL out_index is BG_STATUS_BAD_ARG. */
+int bg_dedup_surfaces_index(const float* surfPos, int B, int S, float threshold, float* out_pos, uint8_t* out_mask,
+                            int32_t* out_index, void* stream);
+/* The trainers' pad_repeat layout (utils.py:100-106) as a gather map, one warp per output row.  src_mask: n_src_rows rows
+ * of in_slots bytes, 1 = padded (as surfMask / edgeM); row_map (int32 [rows], may be NULL = identity): the source row of
+ * each output row, -1 = no source.  out_index (rows, out_slots) int32: the flat source-token index
+ * (src_row * in_slots + slot) each output slot takes when the n valid slots of the source row, in slot order, are
+ * repeated to out_slots.  Every slot of a row without a source or without a valid slot is -1; every slot of a row with
+ * more valid slots than out_slots, or whose row_map entry is outside [-1, n_src_rows), is -2 (which bg_add_noise_gather
+ * poisons).  BG_STATUS_BAD_ARG, launching nothing: NULL src_mask / out_index, rows or n_src_rows <= 0, in_slots outside
+ * [1, 256], out_slots <= 0, rows > n_src_rows without a row map, n_src_rows * in_slots beyond 32 bits. */
+int bg_fill_index(const uint8_t* src_mask, const int32_t* row_map, int64_t rows, int64_t n_src_rows, int32_t in_slots,
+                  int32_t out_slots, int32_t* out_index, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Unit-level entry points (used by tests and the bench to check/time individual kernels through the C ABI).

@@ -55,6 +55,13 @@ run("repaint step", RP.test_step_matches_float64_and_ddim, 18, 13, 0.8, "random"
 run("repaint undo", RP.test_undo_is_the_fp32_chain_bit_for_bit, 50, 300)
 run("repaint forms", RP.test_noise_forms_agree, 6, 7)
 run("repaint bad args", RP.test_bad_arguments_are_rejected_and_launch_nothing)
+import test_gpu_variation as VA   # noqa: E402
+run("variation gather", VA.test_gather_is_the_torch_expression_bit_for_bit, 18, 50, 3.0)
+run("variation keyed gather", VA.test_keyed_z_is_randn_keyed, 18, 13)
+run("variation poisoned gather", VA.test_out_of_range_index_poisons_only_its_token)
+run("variation fill", VA.test_fill_index_matches_oracle, 100, 50, True)
+run("variation dedup index", VA.test_dedup_index_keeps_positions_and_mask, "duplicates", 3, 7)
+run("variation bad args", VA.test_bad_arguments_are_rejected_and_launch_nothing)
 if what != "ops-no-res1":
     run("gemm", T.test_gemm, 128 * 170 + 5, 768, 1024, 0, 0, True, True, 0)   # persistent tiles wrap, residual epilogue
 if what == "all":
