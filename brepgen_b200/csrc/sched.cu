@@ -506,6 +506,69 @@ __global__ void __launch_bounds__(256) axpby_kernel(const float* x, float a, con
     out[i] = a * x[i] + (y ? b * y[i] : 0.f);
 }
 
+// Spherical interpolation of two noises per sample (B-rep interpolation between two DDIM-inverted designs).  One CTA per
+// sample: a.b, |a|^2 and |b|^2 over the elements of unmasked tokens, each thread summing a fixed stride of elements in
+// fp64 and then a fixed shared-memory tree, so the result depends on neither the batch nor the launch; then
+//   theta = acos(clamp(cos, -1, 1)),  out = sin((1-alpha) theta)/sin theta * a + sin(alpha theta)/sin theta * b,
+// or the lerp (1-alpha) a + alpha b when |cos| > 0.9995 or a norm is zero, in fp64 rounded once to fp32.  alpha == 0 and
+// alpha == 1 copy a and b; masked tokens copy a.  Every element is read in the reduction before the barrier and written
+// only after it by the thread that reads it again, so out may alias a.
+constexpr int kSlerpThreads = 512;
+struct SlerpP {
+  const float *a, *b, *alpha;
+  const unsigned char* mask;
+  float* out;
+  long long per_sample, per_token;
+};
+__global__ void __launch_bounds__(kSlerpThreads) slerp_kernel(const SlerpP p) {
+  __shared__ double red[3][kSlerpThreads];
+  const int tid = threadIdx.x;
+  const long long base = (long long)blockIdx.x * p.per_sample;
+  const float* a = p.a + base;
+  const float* b = p.b + base;
+  float* o = p.out + base;
+  const unsigned char* m = p.mask ? p.mask + base / p.per_token : nullptr;
+  const float al = p.alpha[blockIdx.x];
+  double ab = 0.0, aa = 0.0, bb = 0.0;
+  for (long long i = tid; i < p.per_sample; i += kSlerpThreads) {
+    if (m && m[i / p.per_token]) continue;
+    const double x = a[i], y = b[i];
+    ab = fma(x, y, ab);
+    aa = fma(x, x, aa);
+    bb = fma(y, y, bb);
+  }
+  red[0][tid] = ab; red[1][tid] = aa; red[2][tid] = bb;
+  for (int s = kSlerpThreads / 2; s > 0; s >>= 1) {
+    __syncthreads();
+    if (tid < s) {
+      red[0][tid] += red[0][tid + s];
+      red[1][tid] += red[1][tid + s];
+      red[2][tid] += red[2][tid + s];
+    }
+  }
+  __syncthreads();
+  const int mode = al == 0.f ? 0 : (al == 1.f ? 1 : 2);   // copy a, copy b, combine
+  double ca = 1.0 - (double)al, cb = (double)al;          // the lerp
+  if (mode == 2) {
+    const double nn = sqrt(red[1][0] * red[2][0]);
+    const double c = nn > 0.0 ? fmin(fmax(red[0][0] / nn, -1.0), 1.0) : 1.0;
+    if (fabs(c) <= 0.9995) {
+      const double th = acos(c), s = sin(th);
+      ca = sin((1.0 - (double)al) * th) / s;
+      cb = sin((double)al * th) / s;
+    }
+  }
+  for (long long i = tid; i < p.per_sample; i += kSlerpThreads) {
+    const float x = a[i];
+    float v = x;
+    if (!(m && m[i / p.per_token])) {
+      if (mode == 1) v = b[i];
+      else if (mode == 2) v = (float)fma(ca, (double)x, cb * (double)b[i]);
+    }
+    o[i] = v;
+  }
+}
+
 inline unsigned grid_for(long long work) {
   long long blocks = (work + 255) / 256;
   const long long cap = (long long)num_sms() * 16;
@@ -739,6 +802,18 @@ int bg_repaint_undo_tab(float* x, int64_t n, int32_t n_trans, uint64_t seed, con
   UndoP p = {};
   p.x = x; p.n = n; p.n_trans = n_trans; p.seed = seed; p.coef = coef_table; p.step = step;
   return launch_grouped(repaint_undo_kernel, p, sample_keys, per_sample, stream, "repaint_undo_kernel launch");
+}
+
+int bg_slerp(const float* a, const float* b, const float* alpha, const uint8_t* token_mask, int64_t n_samples,
+             int64_t per_sample, int64_t per_token, float* out, void* stream) {
+  BG_REQUIRE(a && b && alpha && out, "slerp: a, b, alpha and out must not be NULL");
+  BG_REQUIRE(n_samples > 0 && n_samples <= 0x7FFFFFFFll && per_sample > 0 && per_token > 0,
+             "slerp: n_samples (at most 2^31 - 1), per_sample and per_token must be positive");
+  BG_REQUIRE(per_sample % per_token == 0, "slerp: per_sample must be a multiple of per_token");
+  SlerpP p;
+  p.a = a; p.b = b; p.alpha = alpha; p.mask = token_mask; p.out = out; p.per_sample = per_sample; p.per_token = per_token;
+  slerp_kernel<<<(unsigned)n_samples, kSlerpThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch("slerp_kernel launch");
 }
 
 int bg_step_advance(const int64_t* timesteps, int n_steps, int32_t* step, int64_t* t_cur, void* stream) {

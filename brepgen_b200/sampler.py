@@ -10,8 +10,9 @@ reshapes (sample.py:284-294).  Differences, all result-preserving:
     (few-step sampling of the same DDPM-trained denoisers), "dpm" = N DPM-Solver++ steps for every stage (the
     second-order multistep sampler of the same denoisers) and "repaint" = diffusers' RePaint list of DDIM-form steps and
     undo steps per stage (resampling, for completion).
-Beyond the reference: completion (known=Completion) and variations (source=Variation: SDEdit, each stage re-noised to a
-chosen strength and denoised again, or kept as given).
+Beyond the reference: completion (known=Completion), variations (source=Variation: SDEdit, each stage re-noised, or
+DDIM-inverted, to a chosen strength and denoised again, or kept as given) and interpolation (source=Interpolation: two
+designs DDIM-inverted, slerped and denoised).
 Everything past sample.py:299 (OpenCASCADE post-processing) is out of scope (SURVEY.md section 2).
 
 Batch sharding across GPUs: samples are independent through every stage, so each rank runs its own shard and there is
@@ -25,8 +26,9 @@ from typing import Dict, List, Optional, Sequence, Tuple, Union
 import torch
 
 from . import _ffi
-from .schedulers import (DPM_ALGORITHMS, DDIMScheduler, DDPMScheduler, DPMSolverMultistepScheduler, PNDMScheduler,
-                         RePaintScheduler, dpm_timesteps, repaint_entries, sample_keys, sample_seed, strength_timesteps)
+from .schedulers import (DPM_ALGORITHMS, DDIMInverseScheduler, DDIMScheduler, DDPMScheduler, DPMSolverMultistepScheduler,
+                         PNDMScheduler, RePaintScheduler, dpm_timesteps, repaint_entries, sample_keys, sample_seed,
+                         strength_timesteps)
 
 NOISE_MODES = ("batch", "per_sample")
 
@@ -260,7 +262,13 @@ class Variation:
     edgePos (B, S, E, 6), edgeM (B, S, E) bool, edge_z (B, S, E, 12), edgeV (B, S, E, 6); S = 2 * num_surfaces without
     CFG, num_surfaces with it; E = num_edges.  strength: one value in [0, 1] for all stages, or four for (surfPos, surfZ,
     edgePos, edgeZV).  1 = a fresh sample, 0 = keep the stage as given (zero strengths must come first: a later stage is
-    conditioned on the earlier ones)."""
+    conditioned on the earlier ones).
+    start: "noise" = the source noised to the tail's first timestep with fresh z (SDEdit); "invert" = the source
+    DDIM-inverted to that timestep (schedule "ddim", ddim_eta 0), deterministic: at strength 1 on every stage the run
+    reconstructs the source.  The inversion runs in the stage's slot layout with the conditioning gathered from the
+    source through the same maps; slots without a source take the stage's z before the inversion.  A non-CFG surfPos
+    stage is inverted at the slots it starts with all the way, while its denoising doubles them at t <= 249 as a plain
+    run does, so there the inversion is not the exact reverse of the denoising."""
     surfPos: torch.Tensor
     surfMask: torch.Tensor
     surfZ: torch.Tensor
@@ -269,12 +277,30 @@ class Variation:
     edge_z: torch.Tensor
     edgeV: torch.Tensor
     strength: Union[float, Sequence[float]] = 1.0
+    start: str = "noise"
 
     @staticmethod
-    def from_outputs(out: Dict[str, torch.Tensor], strength: Union[float, Sequence[float]]) -> "Variation":
+    def from_outputs(out: Dict[str, torch.Tensor], strength: Union[float, Sequence[float]],
+                     start: str = "noise") -> "Variation":
         """a variation of an earlier Cascade.run output: run(cfg, source=Variation.from_outputs(out, 0.5))"""
         return Variation(*(out[k] for k in ("surfPos", "surfMask", "surfZ", "edgePos", "edgeM", "edge_z", "edgeV")),
-                         strength=strength)
+                         strength=strength, start=start)
+
+
+VARIATION_STARTS = ("noise", "invert")
+
+
+@dataclass
+class Interpolation:
+    """Two B-reps to interpolate with Cascade.run(source=...): every stage DDIM-inverts a and b (schedule "ddim",
+    ddim_eta 0) to the first timestep of its tail as one batch, slerps the two noises per sample with weight alpha[b]
+    (bg_slerp: 0 = a, 1 = b) and denoises the result.  a and b are Variations with equal strengths, all > 0 (their
+    `start` is not read); alpha holds one value in [0, 1] per sample.  Each design is laid out by its own pad_repeat fill
+    and carried across the face de-duplication by the same survivor slots, so slot k of a is paired with slot k of b:
+    faces are paired by fill order, not matched geometrically.  Slots without a source (the same in a and b) keep a's."""
+    a: Variation
+    b: Variation
+    alpha: Union[Sequence[float], torch.Tensor]
 
 
 def stage_timesteps(cfg: CascadeConfig) -> torch.Tensor:
@@ -294,6 +320,11 @@ def start_slots(cfg: CascadeConfig, t0: int) -> int:
 
 def check_variation(cfg: CascadeConfig, source: Variation) -> Tuple[float, float, float, float]:
     """raises on a Variation `cfg` cannot run (host checks only: nothing is launched); returns the four stage strengths"""
+    if source.start not in VARIATION_STARTS:
+        raise ValueError(f"Variation.start must be one of {VARIATION_STARTS}, got {source.start!r}")
+    if source.start == "invert" and (cfg.schedule != "ddim" or float(cfg.ddim_eta) != 0.0):
+        raise NotImplementedError(f"DDIM inversion needs schedule 'ddim' with ddim_eta = 0, got {cfg.schedule!r} with "
+                                  f"ddim_eta = {cfg.ddim_eta}: it reverses the deterministic DDIM step")
     if cfg.schedule not in ("ddpm", "ddim", "dpm"):
         raise NotImplementedError(f"variations need schedule 'ddpm', 'ddim' or 'dpm', got {cfg.schedule!r}: the "
                                   "'reference' hybrid starts with PNDM's Runge-Kutta warm-up, and 'repaint' is for completion")
@@ -329,6 +360,8 @@ def check_variation(cfg: CascadeConfig, source: Variation) -> Tuple[float, float
         raise ValueError(f"Variation strengths {st}: zero strengths must come first (a stage is conditioned on the ones "
                          "before it, so it cannot be kept while they change)")
     mask = source.surfMask.cpu()
+    if source.start == "invert" and bool(mask.all(1).any()):
+        raise ValueError(f"Variation: samples {torch.nonzero(mask.all(1)).flatten().tolist()} have no valid face to invert")
     if bool((source.edgeM[..., 0].cpu() & ~mask).any()):
         raise ValueError("Variation.edgeM[..., 0] is set on a valid face: edge slot 0 of a face is always valid")
     if st[0] > 0:
@@ -343,6 +376,30 @@ def check_variation(cfg: CascadeConfig, source: Variation) -> Tuple[float, float
                              f"({nv.max().item()}) than the {slots} face slots a run has at t = {t0}, where a surfPos "
                              f"strength of {st[0]} starts{hint}")
     return tuple(st)
+
+
+def check_interpolation(cfg: CascadeConfig, source: Interpolation) -> Tuple[Tuple[float, ...], torch.Tensor]:
+    """raises on an Interpolation `cfg` cannot run (host checks only: nothing is launched); returns the four stage
+    strengths and alpha as a CPU fp32 tensor"""
+    st = []
+    for name in ("a", "b"):
+        v = getattr(source, name)
+        if not isinstance(v, Variation):
+            raise ValueError(f"Interpolation.{name} must be a Variation, got {type(v).__name__}")
+        try:
+            st.append(check_variation(cfg, replace(v, start="invert")))
+        except ValueError as e:
+            raise ValueError(f"Interpolation.{name}: {e}") from None
+    if st[0] != st[1]:
+        raise ValueError(f"Interpolation: a and b must have equal strengths, got {list(st[0])} and {list(st[1])}")
+    if any(v == 0 for v in st[0]):
+        raise ValueError(f"Interpolation strengths {list(st[0])} must all be > 0: both designs are inverted at every stage")
+    alpha = torch.as_tensor(source.alpha, dtype=torch.float64).cpu().reshape(-1)
+    if alpha.numel() != cfg.batch_size:
+        raise ValueError(f"Interpolation.alpha has {alpha.numel()} values for batch_size {cfg.batch_size}")
+    if not bool(((alpha >= 0) & (alpha <= 1)).all()):
+        raise ValueError(f"Interpolation.alpha must lie in [0, 1], got {alpha.tolist()}")
+    return st[0], alpha.float()
 
 
 def randn_keyed(seeds: Sequence[int], stage: int, shape, device, domain: int = 1, t: int = 0) -> torch.Tensor:
@@ -397,6 +454,20 @@ def fill_index(src_mask: torch.Tensor, out_slots: int, row_map: Optional[torch.T
     return out
 
 
+def slerp(a: torch.Tensor, b: torch.Tensor, alpha: torch.Tensor, token_mask: Optional[torch.Tensor] = None,
+          out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """per-sample spherical interpolation (bg_slerp) of contiguous fp32 a, b (B, ..., D) with weights alpha (B,); tokens
+    are the last dimension; token_mask (B, ...) bool or uint8, True = copied from a; out may be a"""
+    B, D = a.shape[0], a.shape[-1]
+    al = alpha.to(device=a.device, dtype=torch.float32).contiguous()
+    m = None if token_mask is None else token_mask.to(torch.uint8).contiguous()
+    out = torch.empty_like(a) if out is None else out
+    with torch.cuda.device(a.device):
+        _ffi.check(_ffi.lib().bg_slerp(a.data_ptr(), b.data_ptr(), al.data_ptr(), _ffi.ptr(m), B, a.numel() // B, D,
+                                      out.data_ptr(), _ffi.current_stream()), "bg_slerp")
+    return out
+
+
 def dedup_edges(edgePos: torch.Tensor, surfMask: torch.Tensor, threshold: float):
     B, S, E, _ = edgePos.shape
     x = edgePos.float().contiguous()
@@ -423,6 +494,9 @@ class Cascade:
         self.ddim = DDIMScheduler(num_train_timesteps=1000, beta_schedule="linear", prediction_type="epsilon",
                                   beta_start=0.0001, beta_end=0.02, clip_sample=True, clip_sample_range=3,
                                   set_alpha_to_one=True)
+        self.ddim_inv = DDIMInverseScheduler(num_train_timesteps=1000, beta_schedule="linear", prediction_type="epsilon",
+                                             beta_start=0.0001, beta_end=0.02, clip_sample=True, clip_sample_range=3,
+                                             set_alpha_to_one=True)
         self.dpm = self._dpm_scheduler(2, "dpmsolver++")
         self.repaint = RePaintScheduler(num_train_timesteps=1000, beta_schedule="linear", beta_start=0.0001,
                                         beta_end=0.02, clip_sample=True, clip_sample_range=3)
@@ -443,7 +517,8 @@ class Cascade:
         return n_steps >= 32 and tokens <= 100_000
 
     def _loop_graph(self, cfg: CascadeConfig, sched, timesteps, x, fwd, known=None, tables=None):
-        """sched: self.ddpm, self.ddim or self.dpm; timesteps: 1-D int64 CPU tensor; x: (B, ...) fp32 on the device; fwd(x_in, t_dev)
+        """sched: self.ddpm, self.ddim, self.ddim_inv (a DDIMScheduler whose table rows are the inverse step's, sigma = 0)
+        or self.dpm; timesteps: 1-D int64 CPU tensor; x: (B, ...) fp32 on the device; fwd(x_in, t_dev)
         -> eps of a (possibly CFG-doubled) batch.  The loop body of sample.py:145-153 -- [step counter / timestep advance] ->
         forward -> fused scheduler step (CFG combine, x0, clip, DDPM posterior mean or DDIM update, Philox noise) -- is
         captured ONCE and replayed len(timesteps) times: no per-step host work.  Nothing step-specific is a kernel argument:
@@ -540,7 +615,8 @@ class Cascade:
               rnoise_fn=None):
         """fwd(x_in, t_dev) -> eps for a (possibly CFG-doubled) batch; noise_fn(k, shape) -> explicit DDPM / DDIM step noise.
         known: {slots: (values, token mask)} of a completion: the known tokens are replaced before the first step and after
-        every step (sched.replace_known); rnoise_fn(k, shape) -> explicit replacement noise (k = -1 before the first step)."""
+        every step (sched.replace_known); rnoise_fn(k, shape) -> explicit replacement noise (k = -1 before the first step).
+        sched may be self.ddim_inv with its ascending timesteps: a DDIM inversion, run as a DDIM loop that draws nothing."""
         B = x.shape[0]
         k = 0
         fused = isinstance(sched, (DDPMScheduler, DDIMScheduler, DPMSolverMultistepScheduler))   # CFG, noise in the kernel
@@ -612,6 +688,8 @@ class Cascade:
             sde = sched.config.algorithm_type == "sde-dpmsolver++"
             nz = noise_fn(k, x.shape).to(self.device) if (noise_fn is not None and sde) else None
             return sched.step(pred, t, x, generator=gen, variance_noise=nz, **cf).prev_sample
+        if isinstance(sched, DDIMInverseScheduler):
+            return sched.step(pred, t, x, **cf).prev_sample
         if isinstance(sched, DDIMScheduler):
             nz = noise_fn(k, x.shape).to(self.device) if (noise_fn is not None and cfg.ddim_eta > 0) else None
             return sched.step(pred, t, x, eta=cfg.ddim_eta, generator=gen, variance_noise=nz, **cf).prev_sample
@@ -816,13 +894,15 @@ class Cascade:
         return kn
 
     # ------------------------------------------------------------------ variations
-    def _vary_start(self, name, shape, src, index, scale, t0, init_noise, seeds, cpu_gen):
+    def _vary_start(self, name, shape, src, index, scale, t0, init_noise, seeds, cpu_gen, copies=1):
         """the start of a varied stage (bg_add_noise_gather): sa*(scale*src[index]) + sb*z with (sa, sb) of add_noise at
-        t0; index (int32, one per token of `shape`) into the tokens of src, -1 = pure noise.  z: init_noise[name], else the
-        per-sample keys of the stage drawn in the kernel (bg_randn_keyed's initial noise), else the CPU generator."""
+        t0, or (1, 0) when t0 is None (the gathered source itself, which an inversion starts from); index (int32, one per
+        token of `shape`) into the tokens of src, -1 = pure noise.  z: init_noise[name], else the per-sample keys of the
+        stage drawn in the kernel (bg_randn_keyed's initial noise), else the CPU generator.  copies: index holds that many
+        maps of `shape` one after the other, and each copy of the output takes the same z."""
         dev = self.device
         dim = shape[-1]
-        out = torch.empty(shape, dtype=torch.float32, device=dev)
+        out = torch.empty((copies * shape[0],) + tuple(shape[1:]), dtype=torch.float32, device=dev)
         n_tok = out.numel() // dim
         z = keys = None
         if init_noise is not None and name in init_noise:
@@ -833,19 +913,40 @@ class Cascade:
             keys = torch.from_numpy(sample_keys(seeds, self._STAGE_ID[name]).view("int64")).to(dev)
         else:
             z = torch.randn(shape, generator=cpu_gen).to(dev)
-        sa, sb = self.ddpm.replace_coefficients(t0, initial=True)
+        if copies > 1:
+            z, keys = (None if v is None else torch.cat([v] * copies) for v in (z, keys))
+        sa, sb = (1.0, 0.0) if t0 is None else self.ddpm.replace_coefficients(t0, initial=True)
         src = src.reshape(-1, dim)
         idx = index.to(torch.int32).contiguous()
         with torch.cuda.device(dev):
             _ffi.check(_ffi.lib().bg_add_noise_gather(src.data_ptr(), src.shape[0], idx.data_ptr(), n_tok, dim,
-                                                     float(scale), sa, sb, _ffi.ptr(z), _ffi.ptr(keys), n_tok // shape[0],
+                                                     float(scale), sa, sb, _ffi.ptr(z), _ffi.ptr(keys), n_tok // out.shape[0],
                                                      1, 0, out.data_ptr(), _ffi.current_stream()), "bg_add_noise_gather")
         return out
+
+    def _invert_start(self, cfg, name, shape, srcs, maps, scale, tail, fwd, alpha, init_noise, seeds, cpu_gen):
+        """the start of a stage of an inverted variation (one source) or an interpolation (two): every source gathered
+        through its own map (maps: one (B, ...) int32 map per source; -1 slots take the stage's z), DDIM-inverted as one
+        batch along the reversed tail, so that it lands at the tail's first timestep, by fwd(x, t) with the conditioning
+        of that batch; two sources are then slerped with weights alpha, tokens without a source copied from the first."""
+        B = shape[0]
+        off = [0]
+        for s in srcs[:-1]:
+            off.append(off[-1] + s[name].numel() // shape[-1])
+        src = torch.cat([s[name].reshape(-1, shape[-1]) for s in srcs])
+        index = torch.cat([torch.where(i >= 0, i + o, i) for i, o in zip(maps, off)])
+        x = self._vary_start(name, shape, src, index, scale, None, init_noise, seeds, cpu_gen, copies=len(srcs))
+        self.ddim_inv.set_timesteps(cfg.ddim_steps)
+        x = self._loop(cfg, self.ddim_inv, tail.flip(0), x, fwd, None, None)
+        if len(srcs) == 2:
+            x = slerp(x[:B], x[B:], alpha, maps[0] < 0, out=x[:B])
+        return x
 
     # ------------------------------------------------------------------ the cascade
     @torch.no_grad()
     def run(self, cfg: CascadeConfig, init_noise: Optional[Dict[str, torch.Tensor]] = None, step_noise=None,
-            known: Optional[Completion] = None, replace_noise=None, undo_noise=None, source: Optional[Variation] = None):
+            known: Optional[Completion] = None, replace_noise=None, undo_noise=None,
+            source: Optional[Union[Variation, Interpolation]] = None):
         """step_noise(stage_name, k, shape) -> tensor: explicit DDPM / DDIM / DPM step noise of step k (parity runs; DDPM
         draws it at t > 0, DDIM on every step when ddim_eta > 0, DPM on every step of "sde-dpmsolver++"); default = in-kernel
         Philox
@@ -861,7 +962,10 @@ class Cascade:
         stage with strength 0 is not run and returns the source as given, bit for bit.  A varied stage's slots take
         their source tokens in the trainers' pad_repeat layout (bg_fill_index), across the face de-duplication
         (bg_dedup_surfaces_index); slots without a source start from pure noise.  init_noise[name] is the start noise z
-        of a varied stage (shape: the stage's starting shape).
+        of a varied stage (shape: the stage's starting shape).  Variation(start="invert") and source=Interpolation
+        (schedule "ddim", ddim_eta 0): a varied stage starts from its source (both sources) DDIM-inverted along the
+        reversed tail instead (self.ddim_inv through the same loops), then slerped (bg_slerp) for an interpolation; z only
+        fills the slots without a source, so neither draws any other noise.
         schedule "repaint": step_noise(stage_name, k, shape) is the one z of the step at list entry k (drawn at every
         step); undo_noise(stage_name, k, (n, *shape)) the normals of the undo step at entry k.  Known tokens are kept by
         the RePaint step itself (no separate replacement: replace_noise is not used), and known=None is DDIM with
@@ -870,7 +974,12 @@ class Cascade:
         if source is not None and known is not None:
             raise ValueError("Cascade.run: a variation (source=) cannot be combined with a completion (known=)")
         n_known = check_completion(cfg, known) if known is not None else None
-        strength = check_variation(cfg, source) if source is not None else None
+        interp = isinstance(source, Interpolation)
+        alpha = None
+        if interp:
+            strength, alpha = check_interpolation(cfg, source)
+        else:
+            strength = check_variation(cfg, source) if source is not None else None
         seeds = per_sample_seeds(cfg)
         self._sample_seeds = seeds
         dev = self.device
@@ -915,29 +1024,56 @@ class Cascade:
 
         # a variation: the source on the device, the tail of the list each varied stage runs (None: kept), and where the
         # start of each varied stage takes its tokens from (flat source-token indices, -1 = none)
+        # an interpolation: both designs, each with its own maps, inverted as one batch of 2B and slerped
         var = source is not None
-        tails, src = {}, {}
+        sources = [source.a, source.b] if interp else [source]
+        invert = interp or (var and source.start == "invert")
+        tails, srcs = {}, []
         if var:
             full = stage_timesteps(cfg)
             tails = {name: strength_timesteps(full, v) if v > 0 else None for name, v in zip(STAGES, strength)}
-            for k in ("surfPos", "surfZ", "edgePos", "edge_z", "edgeV", "surfMask", "edgeM"):
-                t = getattr(source, k)
-                src[k] = t.to(device=dev, dtype=t.dtype if t.dtype == torch.bool else torch.float32, copy=True).contiguous()
-            src["edgeZV"] = torch.cat([src["edge_z"], src["edgeV"]], -1)
+            for v in sources:
+                s = {}
+                for k in ("surfPos", "surfZ", "edgePos", "edge_z", "edgeV", "surfMask", "edgeM"):
+                    t = getattr(v, k)
+                    s[k] = t.to(device=dev, dtype=t.dtype if t.dtype == torch.bool else torch.float32,
+                                copy=True).contiguous()
+                s["edgeZV"] = torch.cat([s["edge_z"], s["edgeV"]], -1)
+                srcs.append(s)
+        src = srcs[0] if var else {}
         kept = lambda name: var and tails[name] is None
+        label_inv = None
+        if invert and cfg.use_cf:
+            label_inv = torch.tensor([cfg.class_label] * (len(srcs) * B) + [TEXT2INT["uncond"]] * (len(srcs) * B),
+                                     device=dev).reshape(-1, 1)
 
-        def vary(name, shape, index, scale):
-            return self._vary_start(name, shape, src[name], index, scale, int(tails[name][0]), init_noise, seeds, cpu_gen)
+        def take(field, maps, scale=1.0):
+            # the inversion's conditioning: each source's field gathered through its map (0 where -1), one batch
+            return rep2(torch.cat([torch.where((i >= 0)[..., None], s[field].reshape(-1, s[field].shape[-1])[
+                i.long().clamp(min=0)] * scale, 0.0) for s, i in zip(srcs, maps)]))
+
+        def holes(maps):
+            return rep2(torch.cat([i < 0 for i in maps]))
+
+        def vary(name, shape, maps, scale, model, cond=tuple):
+            """maps: one index map per source; model, cond(): the denoiser and its conditioning for an inversion"""
+            if not invert:
+                return self._vary_start(name, shape, src[name], maps[0], scale, int(tails[name][0]), init_noise, seeds,
+                                        cpu_gen)
+            c = cond()
+            return self._invert_start(cfg, name, shape, srcs, maps, scale, tails[name],
+                                      lambda x, t: self.m[model](x, t, *c, label_inv), alpha, init_noise, seeds,
+                                      cpu_gen)
 
         mask_gen = torch.Generator().manual_seed(cfg.seed + 12345)
         if kept("surfPos"):
             surfPos, surfMask = src["surfPos"] * 3.0, src["surfMask"]
-            rows = torch.where(surfMask, -1, torch.arange(B * S, dtype=torch.int32, device=dev).view(B, S))
+            rows = [torch.where(surfMask, -1, torch.arange(B * S, dtype=torch.int32, device=dev).view(B, S))]
         else:
             if var:       # the source's valid faces repeated to the slots a plain run has at the first timestep
                 S1 = start_slots(cfg, int(tails["surfPos"][0]))
-                fill = fill_index(src["surfMask"], S1)
-            surfPos = vary("surfPos", (B, S1, 6), fill, 3.0) if var else noise("surfPos", (B, S0, 6))
+                fill = [fill_index(s["surfMask"], S1) for s in srcs]
+            surfPos = vary("surfPos", (B, S1, 6), fill, 3.0, "surfpos") if var else noise("surfPos", (B, S0, 6))
             surfPos = self._stage(cfg, surfPos, lambda x, t: self.m["surfpos"](x, t, label2), label2, gen, True,
                                   on_step=late_increase, noise_fn=nf("surfPos"), name="surfPos", known=kn.get("surfPos"),
                                   rnoise_fn=rnf("surfPos"), unoise_fn=unf("surfPos"), timesteps=tails.get("surfPos"))
@@ -953,7 +1089,7 @@ class Cascade:
             elif var:     # survivor k came from slot idx[k], which the late increase's repeat took from fill slot idx % S1
                 surfPos, surfMask, idx = dedup_surfaces_index(surfPos, cfg.bbox_threshold)
                 i = idx.long()
-                rows = torch.where(i >= 0, fill.gather(1, i.clamp(min=0) % S1), -1)
+                rows = [torch.where(i >= 0, f.gather(1, i.clamp(min=0) % S1), -1) for f in fill]
             else:
                 surfPos, surfMask = dedup_surfaces(surfPos, cfg.bbox_threshold)
         sP, sM = rep2(surfPos), rep2(surfMask)
@@ -962,7 +1098,8 @@ class Cascade:
         if kept("surfZ"):
             surfZ = src["surfZ"]
         else:
-            surfZ = vary("surfZ", (B, S, 48), rows, 1.0) if var else noise("surfZ", (B, S, 48))
+            surfZ = vary("surfZ", (B, S, 48), rows, 1.0, "surfz", lambda: (take("surfPos", rows, 3.0), holes(rows))) \
+                if var else noise("surfZ", (B, S, 48))
             surfZ = self._stage(cfg, surfZ, lambda x, t: self.m["surfz"](x, t, sP, sM, label2), label2, gen, False,
                                 noise_fn=nf("surfZ"), name="surfZ", known=kn.get("surfZ"), rnoise_fn=rnf("surfZ"),
                                 unoise_fn=unf("surfZ"), timesteps=tails.get("surfZ"))
@@ -971,11 +1108,13 @@ class Cascade:
         # STEP 2-1 edge positions (sample.py:208-236)
         if kept("edgePos"):
             edgePos, edgeM = src["edgePos"] * 3.0, src["edgeM"]
-            edges = torch.arange(B * S * E, dtype=torch.int32, device=dev).view(B, S, E)
+            edges = [torch.arange(B * S * E, dtype=torch.int32, device=dev).view(B, S, E)]
         else:
             if var:       # the valid edges of each face's source face, repeated to E slots
-                edges = fill_index(src["edgeM"], E, rows.flatten()).view(B, S, E)
-            edgePos = vary("edgePos", (B, S, E, 6), edges, 3.0) if var else noise("edgePos", (B, S, E, 6))
+                edges = [fill_index(s["edgeM"], E, r.flatten()).view(B, S, E) for s, r in zip(srcs, rows)]
+            edgePos = vary("edgePos", (B, S, E, 6), edges, 3.0, "edgepos",
+                           lambda: (take("surfPos", rows, 3.0), take("surfZ", rows), holes(rows))) \
+                if var else noise("edgePos", (B, S, E, 6))
             edgePos = self._stage(cfg, edgePos, lambda x, t: self.m["edgepos"](x, t, sP, sZ, sM, label2), label2, gen,
                                   True, noise_fn=nf("edgePos"), name="edgePos", known=kn.get("edgePos"),
                                   rnoise_fn=rnf("edgePos"), unoise_fn=unf("edgePos"), timesteps=tails.get("edgePos"))
@@ -996,7 +1135,9 @@ class Cascade:
         if kept("edgeZV"):
             edgeZV = src["edgeZV"]
         else:
-            edgeZV = vary("edgeZV", (B, S, E, 18), edges, 1.0) if var else noise("edgeZV", (B, S, E, 18))
+            edgeZV = vary("edgeZV", (B, S, E, 18), edges, 1.0, "edgez",
+                          lambda: (take("edgePos", edges, 3.0), take("surfPos", rows, 3.0), take("surfZ", rows),
+                                   holes(edges))) if var else noise("edgeZV", (B, S, E, 18))
             edgeZV = self._stage(cfg, edgeZV, lambda x, t: self.m["edgez"](x, t, eP, sP, sZ, eM, label2), label2, gen,
                                  False, noise_fn=nf("edgeZV"), name="edgeZV", known=kn.get("edgeZV"),
                                  rnoise_fn=rnf("edgeZV"), unoise_fn=unf("edgeZV"), timesteps=tails.get("edgeZV"))

@@ -444,6 +444,69 @@ class DDIMScheduler(_NoiseStreams):
         return self.config.num_train_timesteps
 
 
+class DDIMInverseScheduler(DDIMScheduler):
+    """diffusers 0.27 DDIMInverseScheduler for epsilon-prediction models (DDIM inversion: a design back to the noise that
+    produces it).  timesteps ascend; step(eps, t, x) moves x from level t - ratio up to level t, ratio = 1000 // N, with
+    the model evaluated at the target t (diffusers' inverse pipelines); below the first timestep abar = 1 when
+    set_alpha_to_one, else alphas_cumprod[0].  The step is the DDIM step run upwards, so it is bg_ddim_step with
+    (sqrt(1-abar_cur), sqrt(abar_cur)) of the level below, sqrt_abar_prev = sqrt(abar_t), c_dir = sqrt(1 - abar_t) and
+    sigma = 0: step_coefficients / coefficient_table give those rows, and the Cascade loops run it as a DDIM loop.
+    The constructor takes DDIMScheduler's arguments and supports the same subset."""
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.initial_alpha_cumprod = self.final_alpha_cumprod
+        self.timesteps = torch.from_numpy(np.arange(0, self.config.num_train_timesteps).astype(np.int64))
+
+    def set_timesteps(self, num_inference_steps: int, device=None):
+        n_train = self.config.num_train_timesteps
+        if num_inference_steps > n_train:
+            raise ValueError("num_inference_steps cannot exceed num_train_timesteps")
+        self.num_inference_steps = num_inference_steps
+        ratio = n_train // num_inference_steps                      # timestep_spacing = "leading"
+        ts = (np.arange(0, num_inference_steps) * ratio).round().astype(np.int64)
+        self.timesteps = torch.from_numpy(ts + self.config.steps_offset)
+
+    def step_coefficients(self, t: int, eta: float = 0.0):
+        """(sqrt(1-abar_cur), sqrt(abar_cur), sqrt(abar_t), sqrt(1-abar_t), 0) as Python floats (fp32 arithmetic like
+        diffusers), cur = min(t - ratio, num_train_timesteps - 1): the bg_ddim_step arguments of the inverse step"""
+        if eta != 0.0:
+            raise ValueError(f"DDIM inversion is deterministic: eta must be 0, got {eta}")
+        if self.num_inference_steps is None:
+            raise ValueError("Number of inference steps is 'None', you need to run 'set_timesteps' after creating the "
+                             "scheduler")
+        n_train = self.config.num_train_timesteps
+        cur = min(t - n_train // self.num_inference_steps, n_train - 1)
+        a_cur = self.alphas_cumprod[cur] if cur >= 0 else self.initial_alpha_cumprod
+        a_next = self.alphas_cumprod[t]
+        return float((1 - a_cur) ** 0.5), float(a_cur ** 0.5), float(a_next ** 0.5), float((1 - a_next) ** 0.5), 0.0
+
+    def _abar_prev(self, t: int) -> torch.Tensor:
+        raise NotImplementedError("DDIMInverseScheduler has no known-token replacement")
+
+    def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, return_dict: bool = True,
+             model_output_uncond: Optional[torch.Tensor] = None, guidance_w: float = 0.0,
+             out: Optional[torch.Tensor] = None):
+        """x at level `timestep` from x at the level one step below, and pred_original_sample (the clipped x0 of the
+        step).  Extras over diffusers, as in DDIMScheduler.step: `model_output_uncond` + `guidance_w` fuse the
+        classifier-free combine, `out` is the destination of prev_sample (may be `sample`)."""
+        t = _as_int(timestep)
+        sb, sa, sa_next, c_dir, _ = self.step_coefficients(t)
+        x, eps, eps_u, dst = _step_tensors("DDIMInverseScheduler.step", model_output, sample, model_output_uncond, None,
+                                           out)
+        x0 = torch.empty_like(x)
+        n = x.numel()
+        clip = float(self.config.clip_sample_range) if self.config.clip_sample else 0.0
+        lib = _ffi.lib()
+        with torch.cuda.device(x.device):
+            # x0 first (x may be overwritten next): the same step with sqrt_abar_prev = 1 and c_dir = 0 writes x0 itself
+            for o, c_x0, c_e in ((x0, 1.0, 0.0), (dst, sa_next, c_dir)):
+                _ffi.check(lib.bg_ddim_step(eps.data_ptr(), _ffi.ptr(eps_u), float(guidance_w), x.data_ptr(), o.data_ptr(),
+                                            None, 0, 0, None, n // x.shape[0], t, n, sb, sa, c_x0, c_e, 0.0, clip, 0,
+                                            _ffi.current_stream()), "bg_ddim_step")
+        return SchedulerOutput(dst, x0) if return_dict else (dst, x0)
+
+
 def strength_timesteps(timesteps, strength: float):
     """The tail of a denoising loop that a variation at `strength` runs (diffusers' img2img get_timesteps):
     timesteps[N - min(int(N * strength), N):], N = len(timesteps).  strength 1 is the whole loop, 0 none of it.  The sample

@@ -182,7 +182,10 @@ int bg_randn_keyed(const uint64_t* sample_keys, int64_t n_samples, int64_t per_s
  * noise (only read when sigma != 0): the explicit tensor if not NULL; else, when sample_keys != NULL, the per-sample
  * streams at timestep t (domain 0; the same normals bg_ddpm_step draws at t); else the batch Philox stream (seed, offset)
  * of bg_ddpm_step.  Keyed: per_sample <= 0 or n not a multiple of per_sample is
- * BG_STATUS_BAD_ARG, as are NULL pointers, sqrt_abar <= 0 and t outside 32 bits; nothing is launched then. */
+ * BG_STATUS_BAD_ARG, as are NULL pointers, sqrt_abar <= 0 and t outside 32 bits; nothing is launched then.
+ * The inverse step (DDIM inversion, diffusers DDIMInverseScheduler.step from level t - ratio up to t) is this same call with
+ * (sqrt_one_minus_abar, sqrt_abar) of level t - ratio, sqrt_abar_prev = sqrt(abar_t), c_dir = sqrt(1 - abar_t), sigma = 0
+ * and use_clipped_eps = 0. */
 int bg_ddim_step(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out,
                  const float* noise, uint64_t seed, uint64_t offset, const uint64_t* sample_keys, int64_t per_sample,
                  int64_t t, int64_t n, float sqrt_one_minus_abar, float sqrt_abar, float sqrt_abar_prev, float c_dir,
@@ -292,6 +295,17 @@ int bg_repaint_undo(float* x, int64_t n, int32_t n_trans, const float* coef, con
  * noise.  Bit-identical to bg_repaint_undo with the same coefficients, k and keys or seed. */
 int bg_repaint_undo_tab(float* x, int64_t n, int32_t n_trans, uint64_t seed, const uint64_t* sample_keys,
                         int64_t per_sample, const float* coef_table, const int32_t* step, void* stream);
+/* Spherical interpolation per sample (B-rep interpolation between two DDIM-inverted noises).  a, b, out: n_samples
+ * samples of per_sample fp32 values; alpha: device fp32, one per sample; token_mask: one byte per token of per_token
+ * consecutive values, nonzero = masked (NULL: none masked).  Per sample, a.b, |a|^2 and |b|^2 over the unmasked tokens
+ * (fp64, one CTA per sample, a fixed reduction order: no atomics, independent of the batch), then
+ *   out = sin((1-alpha) theta)/sin(theta) * a + sin(alpha theta)/sin(theta) * b,   theta = acos(clamp(cos, -1, 1)),
+ * or the lerp (1-alpha) a + alpha b when |cos| > 0.9995 or a norm is zero, in fp64 rounded once to fp32.  alpha == 0
+ * gives a and alpha == 1 gives b bit for bit; masked tokens are copied from a.  out may alias a.  No host
+ * synchronisation (graph-capturable).  BG_STATUS_BAD_ARG, launching nothing: NULL a / b / alpha / out, n_samples,
+ * per_sample or per_token <= 0, n_samples >= 2^31, per_sample not a multiple of per_token. */
+int bg_slerp(const float* a, const float* b, const float* alpha, const uint8_t* token_mask, int64_t n_samples,
+             int64_t per_sample, int64_t per_token, float* out, void* stream);
 /* out = c_sample*x - c_eps*(w0*e0 + w1*e1 + w2*e2 + w3*e3)    (PNDM transfer + Adams-Bashforth / RK combination;
  * unused e_i may be NULL with w_i = 0) */
 int bg_pndm_step(const float* x, float* out, int64_t n, float c_sample, float c_eps, const float* e0, float w0,
