@@ -53,6 +53,8 @@ SIGNATURES = {
     "bg_dpm_step": (i32, [vp, vp, f32, vp, vp, vp, vp, u64, u64, vp, i64, i64, i64, f32, f32, f32, f32, f32, f32, f32, f32,
                           vp]),
     "bg_dpm_step_tab": (i32, [vp, vp, f32, vp, vp, vp, u64, u64, u64, vp, i64, vp, i64, vp, vp, f32, vp]),
+    "bg_unipc_step": (i32, [vp, vp, f32, vp, vp, vp, vp, i32, i64, i64, vp, f32, vp]),
+    "bg_unipc_step_tab": (i32, [vp, vp, f32, vp, vp, vp, vp, i64, i64, vp, vp, f32, vp]),
     "bg_replace_known": (i32, [vp, vp, vp, i64, i64, vp, u64, vp, i64, i64, f32, f32, vp]),
     "bg_replace_known_tab": (i32, [vp, vp, vp, i64, i64, u64, vp, i64, vp, vp, vp, vp]),
     "bg_add_noise_gather": (i32, [vp, i64, vp, i64, i32, f32, f32, f32, vp, vp, i64, i32, i64, vp, vp]),

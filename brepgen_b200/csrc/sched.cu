@@ -296,6 +296,86 @@ __global__ void __launch_bounds__(256) dpm_step_kernel(const DpmP p) {
   }
 }
 
+// UniPC multistep step (diffusers UniPCMultistepScheduler, predict_x0, epsilon prediction, "bh1" / "bh2"), one row of
+// BG_UNIPC_ROW coefficients (layout in include/brepgen_b200.h):
+//   x0 = (x - sigma_s*e) / alpha_s, clamped to +-clip;  m_i = hist[slot_i] = x0 of i steps back;
+//   corrector (UniC, corr order c > 0):  xc = cc_x*last - cc_m0*m1 - cc_B*(sum_{i<c} rc_i*(m_{i+1} - m1)/rc_r_i
+//                                                                        + rc_t*(x0 - m1));  else xc = x;
+//   last = xc;  hist[slot_new] = x0;
+//   predictor (UniP, order p):  out = cp_x*xc - cp_m0*x0 - cp_B*sum_{i<p} rp_i*(m_i - x0)/rp_r_i.
+// Every product, quotient and sum is rounded on its own, in diffusers' order (the differences first, the sums left to
+// right), so the step tracks the fp32 torch oracle.  The ring hist (n_slots slots of n elements) and last are read and
+// written in place by the thread that owns the element, all of a group's loads before any store; out may alias x.  The
+// row comes by value (eager form) or from coef[BG_UNIPC_ROW * *step] (table form).  No noise: UniPC is deterministic.
+struct UnipcP {
+  const float *eps_c, *eps_u, *x;
+  float *out, *last, *hist;
+  long long n, per_sample;
+  float w, clip;
+  float row[BG_UNIPC_ROW];
+  const float* coef;
+  const int* step;
+};
+__global__ void __launch_bounds__(256) unipc_step_kernel(const UnipcP p) {
+  const float* r = p.row;
+  if (p.coef) r = p.coef + (long long)BG_UNIPC_ROW * *p.step;
+  const float alpha_s = r[0], sigma_s = r[1];
+  const int corr = (int)r[2], pord = (int)r[3];
+  const long long s_new = (long long)r[4] * p.n;
+  const long long s1 = (long long)r[5] * p.n, s2 = (long long)r[6] * p.n, s3 = (long long)r[7] * p.n;
+  const float cc_x = r[8], cc_m0 = r[9], cc_b = r[10], cr1 = r[11], cr2 = r[12], crho1 = r[13], crho2 = r[14];
+  const float crho_t = r[15];
+  const float cp_x = r[16], cp_m0 = r[17], cp_b = r[18], pr1 = r[19], pr2 = r[20], prho1 = r[21], prho2 = r[22];
+  const int nread = max(corr, pord - 1);     // history slots this step reads: x0 of 1..nread steps back
+  const long long gps = (p.per_sample + 3) / 4, ng = (p.n / p.per_sample) * gps;
+  for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += (long long)gridDim.x * blockDim.x) {
+    const long long b = g / gps, q = g - b * gps;
+    const long long i0 = b * p.per_sample + q * 4;
+    const int cnt = (int)min(4ll, p.per_sample - q * 4);
+    float e[4], xv[4], lv[4] = {0.f, 0.f, 0.f, 0.f}, m1[4] = {0.f, 0.f, 0.f, 0.f}, m2[4] = {0.f, 0.f, 0.f, 0.f},
+        m3[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if (j < cnt) {
+        const long long i = i0 + j;
+        e[j] = p.eps_c[i];
+        if (p.eps_u) e[j] = __fsub_rn(__fmul_rn(e[j], 1.f + p.w), __fmul_rn(p.eps_u[i], p.w));
+        xv[j] = p.x[i];
+        if (corr > 0) lv[j] = p.last[i];
+        if (nread >= 1) m1[j] = p.hist[s1 + i];
+        if (nread >= 2) m2[j] = p.hist[s2 + i];
+        if (nread >= 3) m3[j] = p.hist[s3 + i];
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if (j < cnt) {
+        const long long i = i0 + j;
+        float x0 = __fdiv_rn(__fsub_rn(xv[j], __fmul_rn(sigma_s, e[j])), alpha_s);
+        if (p.clip > 0.f) x0 = fminf(fmaxf(x0, -p.clip), p.clip);
+        float xc = xv[j];
+        if (corr > 0) {
+          float res = 0.f;
+          if (corr >= 2) res = __fmul_rn(crho1, __fdiv_rn(__fsub_rn(m2[j], m1[j]), cr1));
+          if (corr >= 3) res = __fadd_rn(res, __fmul_rn(crho2, __fdiv_rn(__fsub_rn(m3[j], m1[j]), cr2)));
+          const float tail = __fmul_rn(crho_t, __fsub_rn(x0, m1[j]));
+          res = corr >= 2 ? __fadd_rn(res, tail) : tail;
+          xc = __fsub_rn(__fsub_rn(__fmul_rn(cc_x, lv[j]), __fmul_rn(cc_m0, m1[j])), __fmul_rn(cc_b, res));
+        }
+        float o = __fsub_rn(__fmul_rn(cp_x, xc), __fmul_rn(cp_m0, x0));
+        if (pord >= 2) {
+          float res = __fmul_rn(prho1, __fdiv_rn(__fsub_rn(m1[j], x0), pr1));
+          if (pord >= 3) res = __fadd_rn(res, __fmul_rn(prho2, __fdiv_rn(__fsub_rn(m2[j], x0), pr2)));
+          o = __fsub_rn(o, __fmul_rn(cp_b, res));
+        }
+        if (p.last) p.last[i] = xc;
+        p.hist[s_new + i] = x0;
+        p.out[i] = o;
+      }
+    }
+  }
+}
+
 // known[j] = whether the token of element i0 + j (token = element / per_token) has its mask byte set, for j < cnt; returns
 // whether any is.  One division per group of 4: at most 4 mask bytes, usually 1 or 2 distinct.
 __device__ __forceinline__ bool known_flags(const unsigned char* mask, long long i0, long long per_token, int cnt,
@@ -588,6 +668,14 @@ int launch_grouped(void (*kernel)(P), P& p, const uint64_t* sample_keys, int64_t
   return check_launch(what);
 }
 
+// One thread per group of 4 elements of a sample, as launch_grouped; the step draws no noise, so it takes no keys.
+int launch_unipc(UnipcP& p, int64_t per_sample, void* stream) {
+  p.per_sample = per_sample;
+  unipc_step_kernel<<<grid_for((p.n / per_sample) * ((per_sample + 3) / 4)), 256, 0,
+                      reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch("unipc_step_kernel launch");
+}
+
 }  // namespace
 }  // namespace bg
 
@@ -716,6 +804,39 @@ int bg_dpm_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w,
   p.seed = seed; p.offset = offset0; p.offset_stride = offset_stride;
   p.coef = coef_table; p.step = step; p.t_cur = reinterpret_cast<const long long*>(t_cur);
   return launch_grouped(dpm_step_kernel, p, sample_keys, per_sample, stream, "dpm_step_kernel launch");
+}
+
+int bg_unipc_step(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out, float* last,
+                  float* hist, int32_t n_slots, int64_t per_sample, int64_t n, const float* coef, float clip,
+                  void* stream) {
+  BG_REQUIRE(eps_cond && x && out && hist && coef && n > 0, "unipc_step: bad arguments");
+  BG_REQUIRE(per_sample > 0 && n % per_sample == 0, "unipc_step: n must be a positive multiple of per_sample");
+  BG_REQUIRE(n_slots >= 1 && n_slots <= 3, "unipc_step: n_slots must be 1, 2 or 3");
+  BG_REQUIRE(coef[0] > 0.f, "unipc_step: alpha_s must be positive");
+  const float fc = coef[2], fp = coef[3];
+  BG_REQUIRE((fc == 0.f || fc == 1.f || fc == 2.f || fc == 3.f) && (fp == 1.f || fp == 2.f || fp == 3.f),
+             "unipc_step: the corrector order must be 0-3 and the predictor order 1-3");
+  BG_REQUIRE(last || fc == 0.f, "unipc_step: a corrector step needs last");
+  const int reads = max((int)fc, (int)fp - 1);
+  for (int s = 4; s < 8; ++s)
+    BG_REQUIRE(s - 4 > reads || (coef[s] == floorf(coef[s]) && coef[s] >= 0.f && coef[s] < (float)n_slots),
+               "unipc_step: a slot the step uses lies outside the ring of n_slots slots");
+  UnipcP p = {};
+  p.eps_c = eps_cond; p.eps_u = eps_uncond; p.x = x; p.out = out; p.last = last; p.hist = hist; p.n = n;
+  p.w = cfg_w; p.clip = clip;
+  for (int j = 0; j < BG_UNIPC_ROW; ++j) p.row[j] = coef[j];
+  return launch_unipc(p, per_sample, stream);
+}
+
+int bg_unipc_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out, float* last,
+                      float* hist, int64_t per_sample, int64_t n, const float* coef_table, const int32_t* step, float clip,
+                      void* stream) {
+  BG_REQUIRE(eps_cond && x && out && last && hist && coef_table && step && n > 0, "unipc_step_tab: bad arguments");
+  BG_REQUIRE(per_sample > 0 && n % per_sample == 0, "unipc_step_tab: n must be a positive multiple of per_sample");
+  UnipcP p = {};
+  p.eps_c = eps_cond; p.eps_u = eps_uncond; p.x = x; p.out = out; p.last = last; p.hist = hist; p.n = n;
+  p.w = cfg_w; p.clip = clip; p.coef = coef_table; p.step = step;
+  return launch_unipc(p, per_sample, stream);
 }
 
 int bg_replace_known(float* x, const float* known, const uint8_t* token_mask, int64_t n, int64_t per_token,

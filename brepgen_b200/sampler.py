@@ -8,8 +8,9 @@ reshapes (sample.py:284-294).  Differences, all result-preserving:
   * three schedules: "reference" = the shipped PNDM(200)[:158] + DDPM(1000)[-250:] hybrid, "ddpm" = N DDPM steps for
     every stage, which is BASELINE.json's benchmark definition (N = 1000), "ddim" = N DDIM steps for every stage
     (few-step sampling of the same DDPM-trained denoisers), "dpm" = N DPM-Solver++ steps for every stage (the
-    second-order multistep sampler of the same denoisers) and "repaint" = diffusers' RePaint list of DDIM-form steps and
-    undo steps per stage (resampling, for completion).
+    second-order multistep sampler of the same denoisers), "unipc" = N UniPC steps for every stage (predictor-corrector,
+    up to third order) and "repaint" = diffusers' RePaint list of DDIM-form steps and undo steps per stage (resampling,
+    for completion).
 Beyond the reference: completion (known=Completion), variations (source=Variation: SDEdit, each stage re-noised, or
 DDIM-inverted, to a chosen strength and denoised again, or kept as given) and interpolation (source=Interpolation: two
 designs DDIM-inverted, slerped and denoised).
@@ -26,9 +27,9 @@ from typing import Dict, List, Optional, Sequence, Tuple, Union
 import torch
 
 from . import _ffi
-from .schedulers import (DPM_ALGORITHMS, DDIMInverseScheduler, DDIMScheduler, DDPMScheduler, DPMSolverMultistepScheduler,
-                         PNDMScheduler, RePaintScheduler, dpm_timesteps, repaint_entries, sample_keys, sample_seed,
-                         strength_timesteps)
+from .schedulers import (DPM_ALGORITHMS, UNIPC_SOLVER_TYPES, DDIMInverseScheduler, DDIMScheduler, DDPMScheduler,
+                         DPMSolverMultistepScheduler, PNDMScheduler, RePaintScheduler, UniPCMultistepScheduler,
+                         dpm_timesteps, repaint_entries, sample_keys, sample_seed, strength_timesteps)
 
 NOISE_MODES = ("batch", "per_sample")
 
@@ -45,13 +46,16 @@ class CascadeConfig:
     class_label: int = 0                 # TEXT2INT[...] when use_cf
     bbox_threshold: float = 0.08         # eval_config.yaml:10
     guidance_w: float = 0.6              # sample.py:49
-    schedule: str = "reference"          # "reference" | "ddpm" | "ddim" | "dpm" | "repaint"
+    schedule: str = "reference"          # "reference" | "ddpm" | "ddim" | "dpm" | "unipc" | "repaint"
     ddpm_steps: int = 1000               # per stage, schedule == "ddpm"
     ddim_steps: int = 50                 # per stage, schedule == "ddim"
     ddim_eta: float = 0.0                # schedule == "ddim": 0 = deterministic DDIM, 1 = DDPM-like noise
     dpm_steps: int = 20                  # per stage, schedule == "dpm"
     dpm_order: int = 2                   # schedule == "dpm": 1 (DDIM-like) or 2 (DPM-Solver++ 2M)
     dpm_algorithm: str = "dpmsolver++"   # schedule == "dpm": "dpmsolver++" (ODE) or "sde-dpmsolver++" (SDE)
+    unipc_steps: int = 10                # per stage, schedule == "unipc"
+    unipc_order: int = 2                 # schedule == "unipc": predictor order 1, 2 or 3 (the corrector adds one)
+    unipc_solver_type: str = "bh2"       # schedule == "unipc": "bh1" or "bh2" (UniPC's B(h))
     repaint_steps: int = 250             # schedule == "repaint": N of RePaintScheduler.set_timesteps (diffusers' default)
     repaint_eta: float = 0.0             # schedule == "repaint": DDIM eta of the steps
     repaint_jump_length: int = 10        # schedule == "repaint": entries noised back up per jump
@@ -151,8 +155,9 @@ def per_sample_seeds(cfg: CascadeConfig) -> Optional[List[int]]:
 
 def check_schedule(cfg: CascadeConfig) -> None:
     """raises ValueError on out-of-range DDIM settings (ddim_steps outside [1, 1000], ddim_eta < 0), DPM settings
-    (dpm_steps outside [1, 1000], dpm_order not 1 or 2, an unknown dpm_algorithm) and RePaint settings (repaint_steps
-    outside [1, 1000], repaint_eta < 0, repaint_jump_length or repaint_jump_n_sample < 1)"""
+    (dpm_steps outside [1, 1000], dpm_order not 1 or 2, an unknown dpm_algorithm), UniPC settings (unipc_steps outside
+    [1, 1000], unipc_order not 1, 2 or 3, an unknown unipc_solver_type) and RePaint settings (repaint_steps outside
+    [1, 1000], repaint_eta < 0, repaint_jump_length or repaint_jump_n_sample < 1)"""
     if cfg.schedule == "ddim":
         if not 1 <= int(cfg.ddim_steps) <= 1000:
             raise ValueError(f"CascadeConfig.ddim_steps must be in [1, 1000], got {cfg.ddim_steps}")
@@ -165,6 +170,14 @@ def check_schedule(cfg: CascadeConfig) -> None:
             raise ValueError(f"CascadeConfig.dpm_order must be 1 or 2, got {cfg.dpm_order}")
         if cfg.dpm_algorithm not in DPM_ALGORITHMS:
             raise ValueError(f"CascadeConfig.dpm_algorithm must be one of {DPM_ALGORITHMS}, got {cfg.dpm_algorithm!r}")
+    if cfg.schedule == "unipc":
+        if not 1 <= int(cfg.unipc_steps) <= 1000:
+            raise ValueError(f"CascadeConfig.unipc_steps must be in [1, 1000], got {cfg.unipc_steps}")
+        if cfg.unipc_order not in (1, 2, 3):
+            raise ValueError(f"CascadeConfig.unipc_order must be 1, 2 or 3, got {cfg.unipc_order}")
+        if cfg.unipc_solver_type not in UNIPC_SOLVER_TYPES:
+            raise ValueError(f"CascadeConfig.unipc_solver_type must be one of {UNIPC_SOLVER_TYPES}, got "
+                             f"{cfg.unipc_solver_type!r}")
     if cfg.schedule == "repaint":
         if not 1 <= int(cfg.repaint_steps) <= 1000:
             raise ValueError(f"CascadeConfig.repaint_steps must be in [1, 1000], got {cfg.repaint_steps}")
@@ -209,7 +222,7 @@ def check_completion(cfg: CascadeConfig, known: Completion) -> torch.Tensor:
     """raises on a Completion `cfg` cannot run (host checks only; Cascade.run adds the duplicate-face check on the
     device); returns n_faces as a CPU int64 tensor"""
     if cfg.schedule == "reference":
-        raise NotImplementedError("completion needs schedule='ddpm', 'ddim', 'dpm' or 'repaint': PNDM's Runge-Kutta "
+        raise NotImplementedError("completion needs schedule='ddpm', 'ddim', 'dpm', 'unipc' or 'repaint': PNDM's Runge-Kutta "
                                   "steps advance from a sample stored earlier (cur_sample), so known tokens cannot be "
                                   "replaced between them")
     if cfg.dense_masks or cfg.ragged_masks:
@@ -304,9 +317,10 @@ class Interpolation:
 
 
 def stage_timesteps(cfg: CascadeConfig) -> torch.Tensor:
-    """the timestep list every stage of cfg's "ddpm", "ddim" or "dpm" schedule runs (as Cascade.run sets it)"""
-    if cfg.schedule == "dpm":
-        return torch.from_numpy(dpm_timesteps(1000, int(cfg.dpm_steps), "linspace"))
+    """the timestep list every stage of cfg's "ddpm", "ddim", "dpm" or "unipc" schedule runs (as Cascade.run sets it)"""
+    if cfg.schedule in ("dpm", "unipc"):
+        steps = cfg.dpm_steps if cfg.schedule == "dpm" else cfg.unipc_steps
+        return torch.from_numpy(dpm_timesteps(1000, int(steps), "linspace"))
     s = DDIMScheduler() if cfg.schedule == "ddim" else DDPMScheduler()
     s.set_timesteps(int(cfg.ddim_steps if cfg.schedule == "ddim" else cfg.ddpm_steps))
     return s.timesteps
@@ -325,8 +339,8 @@ def check_variation(cfg: CascadeConfig, source: Variation) -> Tuple[float, float
     if source.start == "invert" and (cfg.schedule != "ddim" or float(cfg.ddim_eta) != 0.0):
         raise NotImplementedError(f"DDIM inversion needs schedule 'ddim' with ddim_eta = 0, got {cfg.schedule!r} with "
                                   f"ddim_eta = {cfg.ddim_eta}: it reverses the deterministic DDIM step")
-    if cfg.schedule not in ("ddpm", "ddim", "dpm"):
-        raise NotImplementedError(f"variations need schedule 'ddpm', 'ddim' or 'dpm', got {cfg.schedule!r}: the "
+    if cfg.schedule not in ("ddpm", "ddim", "dpm", "unipc"):
+        raise NotImplementedError(f"variations need schedule 'ddpm', 'ddim', 'dpm' or 'unipc', got {cfg.schedule!r}: the "
                                   "'reference' hybrid starts with PNDM's Runge-Kutta warm-up, and 'repaint' is for completion")
     if cfg.dense_masks or cfg.ragged_masks:
         raise ValueError("variations run the de-duplication; dense_masks and ragged_masks are benchmark modes")
@@ -498,6 +512,7 @@ class Cascade:
                                              beta_start=0.0001, beta_end=0.02, clip_sample=True, clip_sample_range=3,
                                              set_alpha_to_one=True)
         self.dpm = self._dpm_scheduler(2, "dpmsolver++")
+        self.unipc = self._unipc_scheduler(2, "bh2")
         self.repaint = RePaintScheduler(num_train_timesteps=1000, beta_schedule="linear", beta_start=0.0001,
                                         beta_end=0.02, clip_sample=True, clip_sample_range=3)
 
@@ -506,6 +521,13 @@ class Cascade:
         return DPMSolverMultistepScheduler(num_train_timesteps=1000, beta_schedule="linear", prediction_type="epsilon",
                                            beta_start=0.0001, beta_end=0.02, solver_order=order,
                                            algorithm_type=algorithm, clip_sample=True, clip_sample_range=3)
+
+    @staticmethod
+    def _unipc_scheduler(order: int, solver_type: str) -> UniPCMultistepScheduler:
+        # final sigma 0: every stage ends on its data prediction, as the DDIM and DPM stages do
+        return UniPCMultistepScheduler(num_train_timesteps=1000, beta_schedule="linear", prediction_type="epsilon",
+                                       beta_start=0.0001, beta_end=0.02, solver_order=order, solver_type=solver_type,
+                                       final_sigmas_type="zero", clip_sample=True, clip_sample_range=3)
 
     # ------------------------------------------------------------------ one DDPM loop as a replayed CUDA graph
     def _use_graph(self, cfg: CascadeConfig, n_steps: int, tokens: int) -> bool:
@@ -526,8 +548,8 @@ class Cascade:
         (bg_step_advance / bg_ddpm_step_tab / bg_ddim_step_tab / bg_dpm_step_tab), and per-sample noise from the keys at
         the device timestep.  known: {slots: (values, token mask)} of a completion; bg_replace_known_tab then follows the
         step inside the captured body.  tables: (step coefficients, replacement coefficients) of this segment, required for
-        self.dpm, whose rows depend on the whole loop; its history buffer `hist` lives in the scheduler, so it carries over
-        from one segment to the next."""
+        self.dpm and self.unipc, whose rows depend on the whole loop; their history buffer `hist` (and UniPC's corrected
+        sample `last`) lives in the scheduler, so it carries over from one segment to the next."""
         dev = self.device
         lib = _ffi.lib()
         T = len(timesteps)
@@ -536,9 +558,13 @@ class Cascade:
         n = xb.numel()
         ddim = isinstance(sched, DDIMScheduler)
         dpm = isinstance(sched, DPMSolverMultistepScheduler)
+        unipc = isinstance(sched, UniPCMultistepScheduler)
         if dpm:
             coef = tables[0].to(dev)
             hist = sched.history(xb)
+        elif unipc:
+            coef = tables[0].to(dev)
+            hist, last = sched.buffers(xb)
         else:
             coef = (sched.coefficient_table(timesteps, cfg.ddim_eta) if ddim else sched.coefficient_table(timesteps)).to(dev)
         ts = timesteps.to(device=dev, dtype=torch.int64).contiguous()
@@ -553,7 +579,7 @@ class Cascade:
         clip = float(sched.config.clip_sample_range) if sched.config.clip_sample else 0.0
         if known is not None:
             kn, km = known[xb.shape[1]]
-            rtab = (tables[1] if dpm else sched.replace_table(timesteps)).to(dev)
+            rtab = (tables[1] if (dpm or unipc) else sched.replace_table(timesteps)).to(dev)
             rseed = 0 if keyed else sched.replace_seed()
 
         def replace(st):
@@ -573,6 +599,10 @@ class Cascade:
                                                xb.data_ptr(), hist.data_ptr(), seed, off0, stride, _ffi.ptr(keys), n // B,
                                                t_cur.data_ptr(), n, coef.data_ptr(), step.data_ptr(), clip, st),
                            "bg_dpm_step_tab")
+            elif unipc:
+                _ffi.check(lib.bg_unipc_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(),
+                                                 xb.data_ptr(), last.data_ptr(), hist.data_ptr(), n // B, n,
+                                                 coef.data_ptr(), step.data_ptr(), clip, st), "bg_unipc_step_tab")
             elif ddim:
                 _ffi.check(lib.bg_ddim_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(),
                                                 xb.data_ptr(), seed, off0, stride, _ffi.ptr(keys), n // B, t_cur.data_ptr(),
@@ -585,15 +615,18 @@ class Cascade:
 
         # warm-up outside the capture (packs the weights, allocates the workspace), then rewind the state it touched
         x0 = xb.clone()
-        h0 = hist.clone() if dpm else None
+        h0 = hist.clone() if (dpm or unipc) else None
+        last0 = last.clone() if unipc else None
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):
             body()
         torch.cuda.current_stream(dev).wait_stream(side)
         xb.copy_(x0)
-        if dpm:
+        if dpm or unipc:
             hist.copy_(h0)
+        if unipc:
+            last.copy_(last0)
         step.fill_(-1)
         g = torch.cuda.CUDAGraph()
         l0 = lib.bg_launch_count()
@@ -603,8 +636,8 @@ class Cascade:
         for _ in range(T):
             g.replay()
         _ffi.note_replay(per_replay, T)
-        # DDIM draws (and advances the stream) only when eta > 0, DPM-Solver++ only in its SDE form
-        draws = cfg.ddim_eta > 0 if ddim else (sched.config.algorithm_type == "sde-dpmsolver++" if dpm else True)
+        # DDIM draws (and advances the stream) only when eta > 0, DPM-Solver++ only in its SDE form, UniPC never
+        draws = cfg.ddim_eta > 0 if ddim else (sched.config.algorithm_type == "sde-dpmsolver++" if dpm else not unipc)
         if not keyed and draws:
             sched.advance_philox(n, T)
         self.last_graph_steps = getattr(self, "last_graph_steps", 0) + T
@@ -619,7 +652,8 @@ class Cascade:
         sched may be self.ddim_inv with its ascending timesteps: a DDIM inversion, run as a DDIM loop that draws nothing."""
         B = x.shape[0]
         k = 0
-        fused = isinstance(sched, (DDPMScheduler, DDIMScheduler, DPMSolverMultistepScheduler))   # CFG, noise in the kernel
+        fused = isinstance(sched, (DDPMScheduler, DDIMScheduler, DPMSolverMultistepScheduler,   # CFG, noise in the kernel
+                                   UniPCMultistepScheduler))
         if known is not None and len(timesteps) > 0:
             x = self._replace(sched, known, x, timesteps[0], -1, rnoise_fn, initial=True)
         if fused and noise_fn is None and rnoise_fn is None and gen is None and len(timesteps) > 0 and \
@@ -637,9 +671,10 @@ class Cascade:
                 else:
                     hi = len(ts_list)
                 tabs = None
-                if isinstance(sched, DPMSolverMultistepScheduler):
-                    # each segment starts the solver (first order): the loop's first step, a variation's truncated list
-                    # starting mid-table, and a segment after the late increase; rows depend on the whole loop
+                if isinstance(sched, (DPMSolverMultistepScheduler, UniPCMultistepScheduler)):
+                    # each segment starts the solver (first order, no UniPC corrector): the loop's first step, a
+                    # variation's truncated list starting mid-table, and a segment after the late increase; rows depend
+                    # on the whole loop
                     tabs = (sched.coefficient_table(timesteps, restart=lo)[lo:hi],
                             sched.replace_table(timesteps)[lo:hi])
                 x = self._loop_graph(cfg, sched, timesteps[lo:hi], x, fwd, known, tabs)
@@ -682,8 +717,10 @@ class Cascade:
         return sched.replace_known(x, kn, km, t, noise=nz, out=None if initial else x, initial=initial)
 
     def _fused_step(self, cfg, sched, k, t, x, pred, gen, noise_fn, **cf):
-        """one DDPM, DDIM or DPM-Solver++ step; explicit noise from noise_fn on the steps where diffusers draws it: DDPM at
-        t > 0, DDIM on every step when eta > 0, DPM-Solver++ on every step of its SDE form"""
+        """one DDPM, DDIM, DPM-Solver++ or UniPC step; explicit noise from noise_fn on the steps where diffusers draws it:
+        DDPM at t > 0, DDIM on every step when eta > 0, DPM-Solver++ on every step of its SDE form, UniPC never"""
+        if isinstance(sched, UniPCMultistepScheduler):
+            return sched.step(pred, t, x, **cf).prev_sample
         if isinstance(sched, DPMSolverMultistepScheduler):
             sde = sched.config.algorithm_type == "sde-dpmsolver++"
             nz = noise_fn(k, x.shape).to(self.device) if (noise_fn is not None and sde) else None
@@ -812,12 +849,16 @@ class Cascade:
     def _stage(self, cfg, x, fwd, label2, gen, hybrid_ddpm_tail: bool, on_step=None, noise_fn=None, name="surfPos",
                known=None, rnoise_fn=None, unoise_fn=None, timesteps=None):
         """one stage's denoising loop from x; timesteps: a tail of the schedule's list to run instead of all of it (a
-        variation; schedules "ddpm", "ddim" and "dpm")"""
+        variation; schedules "ddpm", "ddim", "dpm" and "unipc")"""
         seeds = getattr(self, "_sample_seeds", None)
         if cfg.schedule == "dpm" and (self.dpm.config.solver_order, self.dpm.config.algorithm_type) != \
                 (cfg.dpm_order, cfg.dpm_algorithm):
             self.dpm = self._dpm_scheduler(cfg.dpm_order, cfg.dpm_algorithm)
-        noisy = {"ddim": self.ddim, "dpm": self.dpm, "repaint": self.repaint}.get(cfg.schedule, self.ddpm)
+        if cfg.schedule == "unipc" and (self.unipc.config.solver_order, self.unipc.config.solver_type) != \
+                (cfg.unipc_order, cfg.unipc_solver_type):
+            self.unipc = self._unipc_scheduler(cfg.unipc_order, cfg.unipc_solver_type)
+        noisy = {"ddim": self.ddim, "dpm": self.dpm, "unipc": self.unipc, "repaint": self.repaint}.get(cfg.schedule,
+                                                                                                      self.ddpm)
         if seeds is not None:
             noisy.set_sample_keys(sample_seeds=seeds, stage=self._STAGE_ID[name])
         else:
@@ -830,6 +871,10 @@ class Cascade:
             self.dpm.set_timesteps(cfg.dpm_steps)
             ts = self.dpm.timesteps if timesteps is None else timesteps
             return self._loop(cfg, self.dpm, ts, x, fwd, label2, gen, on_step, noise_fn, known, rnoise_fn)
+        if cfg.schedule == "unipc":
+            self.unipc.set_timesteps(cfg.unipc_steps)
+            ts = self.unipc.timesteps if timesteps is None else timesteps
+            return self._loop(cfg, self.unipc, ts, x, fwd, label2, gen, on_step, noise_fn, known, rnoise_fn)
         if cfg.schedule == "repaint":
             self.repaint.eta = float(cfg.repaint_eta)
             self.repaint.set_timesteps(cfg.repaint_steps, cfg.repaint_jump_length, cfg.repaint_jump_n_sample)
@@ -953,11 +998,11 @@ class Cascade:
         keyed by (cfg.seed, rank, stage): reproducible from cfg.seed, independent across ranks and stages.
         cfg.noise == "per_sample": initial and step noise come from each sample's own streams (bg_randn_keyed and the fused
         steps' sample keys), so sample b's outputs depend on its seed alone; init_noise / step_noise still take precedence.
-        known: a Completion (schedules "ddpm", "ddim" and "dpm"): every stage that has known tokens replaces them before its
+        known: a Completion (schedules "ddpm", "ddim", "dpm" and "unipc"): every stage that has known tokens replaces them before its
         first step and after every step with the known values noised to the step's level, so the rest is generated
         around them; the known parts come out as given, bit for bit.  replace_noise(stage_name, k, shape) -> tensor:
         explicit noise of that replacement (k = -1 before the first step; parity runs), mirroring step_noise.
-        source: a Variation (schedules "ddpm", "ddim" and "dpm"; not with known): each stage with strength s > 0 starts
+        source: a Variation (schedules "ddpm", "ddim", "dpm" and "unipc"; not with known): each stage with strength s > 0 starts
         from its source noised to the first timestep of strength_timesteps(list, s) and runs that tail of the list; a
         stage with strength 0 is not run and returns the source as given, bit for bit.  A varied stage's slots take
         their source tokens in the trainers' pad_repeat layout (bg_fill_index), across the face de-duplication

@@ -1,6 +1,6 @@
-"""Drop-in DDPMScheduler / PNDMScheduler with the diffusers 0.27 interface used by the reference, DDIMScheduler and
-DPMSolverMultistepScheduler (diffusers' few-step samplers for the same epsilon-prediction models) and RePaintScheduler
-(diffusers' inpainting with resampling; none of these three is used by the reference).
+"""Drop-in DDPMScheduler / PNDMScheduler with the diffusers 0.27 interface used by the reference, DDIMScheduler,
+DPMSolverMultistepScheduler and UniPCMultistepScheduler (diffusers' few-step samplers for the same epsilon-prediction
+models) and RePaintScheduler (diffusers' inpainting with resampling; none of these four is used by the reference).
 
 Call sites mirrored (all in the reference): constructors sample.py:101-117 and trainer.py:285-292;
 `set_timesteps(n)` + `.timesteps[...]` slicing sample.py:128-129,144-145; `.step(pred, t, x).prev_sample`
@@ -8,7 +8,7 @@ sample.py:137,153,202,222,236,282; `.add_noise(x, noise, t)` trainer.py:348; `.c
 
 Host side (this file): the beta / alphas_cumprod tables and the per-step scalar coefficients, computed with the same
 fp32 torch-CPU operations diffusers uses (SURVEY.md Appendix A.3/A.4).  Device side: ONE fused kernel per step
-(bg_ddpm_step / bg_ddim_step / bg_dpm_step / bg_repaint_step / bg_pndm_step in csrc/sched.cu) instead of ~15 scalar-broadcast launches.  No CPU tensor path:
+(bg_ddpm_step / bg_ddim_step / bg_dpm_step / bg_unipc_step / bg_repaint_step / bg_pndm_step in csrc/sched.cu) instead of ~15 scalar-broadcast launches.  No CPU tensor path:
 `step` on a CPU sample raises.
 """
 from __future__ import annotations
@@ -777,6 +777,14 @@ def dpm_timesteps(num_train_timesteps: int, num_inference_steps: int, spacing: s
     raise NotImplementedError(f"timestep_spacing={spacing!r}")
 
 
+def dpm_sigmas(alphas_cumprod: torch.Tensor, timesteps: np.ndarray, sigma_last) -> torch.Tensor:
+    """fp32 sigma table of DPMSolverMultistepScheduler / UniPCMultistepScheduler.set_timesteps: sqrt((1 - abar) / abar)
+    interpolated at the timesteps, then sigma_last appended"""
+    sig = (((1 - alphas_cumprod) / alphas_cumprod) ** 0.5).numpy()
+    sig = np.interp(timesteps, np.arange(0, len(sig)), sig)
+    return torch.from_numpy(np.concatenate([sig, [sigma_last]]).astype(np.float32))
+
+
 class DPMSolverMultistepScheduler(_NoiseStreams):
     """diffusers 0.27 DPMSolverMultistepScheduler for epsilon-prediction models: the DPM-Solver++ multistep ("2M") sampler,
     deterministic ("dpmsolver++") or stochastic ("sde-dpmsolver++"), of a model trained as a DDPM.  One fused kernel per
@@ -846,9 +854,7 @@ class DPMSolverMultistepScheduler(_NoiseStreams):
         if num_inference_steps > n_train:
             raise ValueError("num_inference_steps cannot exceed num_train_timesteps")
         ts = dpm_timesteps(n_train, num_inference_steps, self.config.timestep_spacing, self.config.steps_offset)
-        sig = (((1 - self.alphas_cumprod) / self.alphas_cumprod) ** 0.5).numpy()
-        sig = np.interp(ts, np.arange(0, len(sig)), sig)
-        self.sigmas = torch.from_numpy(np.concatenate([sig, [0]]).astype(np.float32))
+        self.sigmas = dpm_sigmas(self.alphas_cumprod, ts, 0)
         self.timesteps = torch.from_numpy(ts).to(dtype=torch.int64)
         self.num_inference_steps = len(ts)
         self.lower_order_nums = 0
@@ -977,6 +983,240 @@ class DPMSolverMultistepScheduler(_NoiseStreams):
                                              dst.data_ptr(), hist.data_ptr(), _ffi.ptr(noise), seed, offset,
                                              _ffi.ptr(keys), n // x.shape[0], t, n, *coefs, clip, _ffi.current_stream()),
                        "bg_dpm_step")
+        if self.lower_order_nums < self.config.solver_order:
+            self.lower_order_nums += 1
+        self._step_index += 1
+        return SchedulerOutput(dst) if return_dict else (dst,)
+
+    def add_noise(self, original_samples, noise, timesteps):
+        return DDPMScheduler.add_noise(self, original_samples, noise, timesteps)
+
+    def __len__(self):
+        return self.config.num_train_timesteps
+
+
+UNIPC_SOLVER_TYPES = ("bh1", "bh2")
+UNIPC_ROW = 24           # floats per coefficient row (BG_UNIPC_ROW in include/brepgen_b200.h)
+
+
+class UniPCMultistepScheduler(_NoiseStreams):
+    """diffusers' UniPCMultistepScheduler (Zhao et al. 2023) for epsilon-prediction models, in its data-prediction form
+    (predict_x0=True): a predictor (UniP) of order 1-3 and a corrector (UniC) that refines the previous step's output with
+    the data prediction of this step's network evaluation, so no extra evaluation.  One fused kernel per step
+    (bg_unipc_step); the per-step scalars are computed here in fp32 torch as diffusers computes them.  The data
+    predictions (diffusers' model_outputs) live in a device ring `hist` of solver_order slots, and the corrected sample
+    (diffusers' last_sample) in the device tensor `last`; the kernel reads and rewrites both in place.
+
+    final_sigmas_type: "sigma_min" (the default: diffusers 0.27, which has no such parameter, ends at the smallest
+    training sigma) or "zero" (later releases' default: the last step lands on the data prediction).  Under "zero" the
+    last step's first-order predictor is computed as its limit, x0 (diffusers evaluates B(h) * 0 there, inf * 0 under
+    bh1); a predictor of order >= 2 into sigma = 0 has no finite limit (its (m_i - m0) / r_i terms grow like h), so
+    "zero" with lower_order_final=False and solver_order >= 2 raises NotImplementedError.
+
+    Extras over diffusers: `clip_sample` / `clip_sample_range` clamp the data prediction before it is used and stored
+    (off by default), the fused classifier-free combine (`model_output_uncond` + `guidance_w`), `out=`, and the tables of
+    the graph form.  A `step` on a sample whose shape differs from the state's restarts the solver: that step is first
+    order, has no corrector, and the buffers are reallocated."""
+
+    def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.0001, beta_end: float = 0.02,
+                 beta_schedule: str = "linear", trained_betas=None, solver_order: int = 2,
+                 prediction_type: str = "epsilon", thresholding: bool = False, dynamic_thresholding_ratio: float = 0.995,
+                 sample_max_value: float = 1.0, predict_x0: bool = True, solver_type: str = "bh2",
+                 lower_order_final: bool = True, disable_corrector=(), solver_p=None, use_karras_sigmas: bool = False,
+                 timestep_spacing: str = "linspace", steps_offset: int = 0, final_sigmas_type: str = "sigma_min",
+                 clip_sample: bool = False, clip_sample_range: float = 1.0, **unused):
+        if solver_type in ("midpoint", "heun", "logrho"):
+            solver_type = "bh2"           # diffusers' mapping of DPM-Solver's solver types
+        if prediction_type != "epsilon" or not predict_x0 or solver_p is not None or thresholding or \
+                use_karras_sigmas or trained_betas is not None or solver_order not in (1, 2, 3) or \
+                solver_type not in UNIPC_SOLVER_TYPES or final_sigmas_type not in ("sigma_min", "zero") or \
+                timestep_spacing not in ("linspace", "leading", "trailing"):
+            raise NotImplementedError("only prediction_type='epsilon', predict_x0=True, solver_order 1-3, solver_type "
+                                      "'bh1' / 'bh2', final_sigmas_type 'sigma_min' / 'zero', timestep_spacing "
+                                      "'linspace' / 'leading' / 'trailing'; no solver_p, thresholding, Karras sigmas or "
+                                      "trained_betas")
+        if final_sigmas_type == "zero" and not lower_order_final and solver_order >= 2:
+            raise NotImplementedError("final_sigmas_type='zero' with lower_order_final=False: the last predictor would be "
+                                      "of order >= 2 into sigma = 0, which has no finite value")
+        self.config = SimpleNamespace(num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
+                                      beta_schedule=beta_schedule, trained_betas=trained_betas, solver_order=solver_order,
+                                      prediction_type=prediction_type, thresholding=thresholding,
+                                      dynamic_thresholding_ratio=dynamic_thresholding_ratio,
+                                      sample_max_value=sample_max_value, predict_x0=predict_x0, solver_type=solver_type,
+                                      lower_order_final=lower_order_final, disable_corrector=list(disable_corrector),
+                                      solver_p=solver_p, use_karras_sigmas=use_karras_sigmas,
+                                      timestep_spacing=timestep_spacing, steps_offset=steps_offset,
+                                      final_sigmas_type=final_sigmas_type, clip_sample=clip_sample,
+                                      clip_sample_range=clip_sample_range)
+        self.betas = _betas(num_train_timesteps, beta_start, beta_end, beta_schedule)
+        self.alphas = 1.0 - self.betas
+        self.alphas_cumprod = torch.cumprod(self.alphas, dim=0)
+        self.alpha_t = torch.sqrt(self.alphas_cumprod)
+        self.sigma_t = torch.sqrt(1 - self.alphas_cumprod)
+        self.lambda_t = torch.log(self.alpha_t) - torch.log(self.sigma_t)
+        self.sigmas = ((1 - self.alphas_cumprod) / self.alphas_cumprod) ** 0.5
+        self.init_noise_sigma = 1.0
+        self.num_inference_steps = None
+        self.timesteps = torch.from_numpy(np.linspace(0, num_train_timesteps - 1, num_train_timesteps,
+                                                      dtype=np.float32)[::-1].copy())
+        self.hist = self.last = None
+        self._restart()
+        self._step_index = None
+        self._init_noise_streams()
+
+    def _restart(self):
+        self.lower_order_nums = 0
+        self.this_order = None
+        self._has_last = False
+
+    @property
+    def step_index(self):
+        return self._step_index
+
+    @property
+    def model_outputs(self):
+        """diffusers' history list, oldest first: the ring slots of the last lower_order_nums data predictions"""
+        R, k, n = self.config.solver_order, self._step_index, self.lower_order_nums
+        return [None] * (R - n) + [self.hist[(k - i) % R] for i in range(n, 0, -1)]
+
+    @property
+    def last_sample(self):
+        return self.last if self._has_last else None
+
+    def set_timesteps(self, num_inference_steps: int, device=None):
+        n_train = self.config.num_train_timesteps
+        if num_inference_steps > n_train:
+            raise ValueError("num_inference_steps cannot exceed num_train_timesteps")
+        ts = dpm_timesteps(n_train, num_inference_steps, self.config.timestep_spacing, self.config.steps_offset)
+        a0 = self.alphas_cumprod[0]
+        self.sigmas = dpm_sigmas(self.alphas_cumprod, ts,
+                                 float(((1 - a0) / a0) ** 0.5) if self.config.final_sigmas_type == "sigma_min" else 0)
+        self.timesteps = torch.from_numpy(ts).to(dtype=torch.int64)
+        self.num_inference_steps = len(ts)
+        self._restart()
+        self._step_index = None
+
+    scale_model_input = DPMSolverMultistepScheduler.scale_model_input
+    index_for_timestep = DPMSolverMultistepScheduler.index_for_timestep
+    _alpha_sigma = DPMSolverMultistepScheduler._alpha_sigma
+    _abar_after = DPMSolverMultistepScheduler._abar_after
+    _abar_prev = DPMSolverMultistepScheduler._abar_prev
+    replace_table = DPMSolverMultistepScheduler.replace_table
+
+    def _uni(self, s0: int, order: int, corrector: bool) -> list:
+        """(c_x, c_m0, c_B, r_1, r_2, rho_1, rho_2[, rho_t]) of the update from sigmas[s0] to sigmas[s0 + 1] with the data
+        predictions at s0, s0 - 1, ..: diffusers' multistep_uni_c_bh_update (corrector) or multistep_uni_p_bh_update"""
+        alpha_t, sigma_t, lambda_t = self._alpha_sigma(s0 + 1)
+        alpha_s0, sigma_s0, lambda_s0 = self._alpha_sigma(s0)
+        h = lambda_t - lambda_s0
+        rks = [(self._alpha_sigma(s0 - i)[2] - lambda_s0) / h for i in range(1, order)]
+        hh = -h
+        h_phi_1 = torch.expm1(hh)
+        h_phi_k = h_phi_1 / hh - 1
+        factorial_i = 1
+        B_h = hh if self.config.solver_type == "bh1" else torch.expm1(hh)
+        rk = torch.tensor(rks + [1.0])
+        R, b = [], []
+        for i in range(1, order + 1):
+            R.append(torch.pow(rk, i - 1))
+            b.append(h_phi_k * factorial_i / B_h)
+            factorial_i *= i + 1
+            h_phi_k = h_phi_k / hh - 1 / factorial_i
+        R, b = torch.stack(R), torch.tensor(b)
+        if corrector:
+            rhos = [0.5] if order == 1 else torch.linalg.solve(R, b).tolist()
+            hist_rhos, tail = rhos[:-1], [float(rhos[-1])]
+        else:
+            hist_rhos = [] if order == 1 else ([0.5] if order == 2 else torch.linalg.solve(R[:-1, :-1], b[:-1]).tolist())
+            tail = []
+        c_b = float(alpha_t * B_h) if (corrector or order >= 2) else 0.0     # unused by a first-order predictor
+        pad = lambda v: [float(u) for u in v] + [0.0] * (2 - len(v))
+        return [float(sigma_t / sigma_s0), float(alpha_t * h_phi_1), c_b] + pad(rks) + pad(hist_rhos) + tail
+
+    def step_row(self, k: int, corr_order: int, order: int) -> list:
+        """the BG_UNIPC_ROW floats of step index k with a corrector of order corr_order (0: none) and a predictor of order
+        `order` (layout in include/brepgen_b200.h); the x0 of step j sits in ring slot j % solver_order"""
+        R = self.config.solver_order
+        alpha_s, sigma_s, _ = self._alpha_sigma(k)
+        row = [float(alpha_s), float(sigma_s), float(corr_order), float(order)]
+        row += [float((k - i) % R) for i in range(4)]
+        row += self._uni(k - 1, corr_order, True) if corr_order else [0.0] * 8
+        row += self._uni(k, order, False) + [0.0]
+        return row
+
+    def _order(self, k: int, lower_order_nums: int) -> int:
+        """diffusers' this_order of step k: min(solver_order, N - k) with lower_order_final, capped by the warm-up"""
+        R = self.config.solver_order
+        order = min(R, len(self.timesteps) - k) if self.config.lower_order_final else R
+        return min(order, lower_order_nums + 1)
+
+    def _corrects(self, k: int, has_last: bool) -> bool:
+        return k > 0 and (k - 1) not in self.config.disable_corrector and has_last
+
+    def step_plan(self, k0: int, T: int, restart: Optional[int] = None):
+        """[(corrector order, predictor order)] of steps k0 .. k0 + T - 1 of a loop that starts the solver (empty history,
+        no last_sample) at its first step and again at step k0 + restart"""
+        if self.num_inference_steps is None:
+            raise ValueError("Number of inference steps is 'None', you need to run 'set_timesteps' after creating the "
+                             "scheduler")
+        plan, nums, prev, has_last = [], 0, None, False
+        for j in range(T):
+            if j == restart:
+                nums, prev, has_last = 0, None, False
+            k = k0 + j
+            c = prev if self._corrects(k, has_last) else 0
+            p = self._order(k, nums)
+            plan.append((c, p))
+            prev, has_last, nums = p, True, min(nums + 1, self.config.solver_order)
+        return plan
+
+    def coefficient_table(self, timesteps=None, restart: Optional[int] = None) -> torch.Tensor:
+        """[len(timesteps), BG_UNIPC_ROW] fp32 (CPU): step_row of every step of a loop over `timesteps` (default the whole
+        table; a consecutive run of it) planned by step_plan(k0, T, restart) -- the device table that bg_unipc_step_tab
+        indexes with its step counter when the loop is captured in a CUDA graph.  A row depends on the orders of the
+        steps before it, so a loop split into graph segments slices the table of the whole loop."""
+        k0 = 0 if timesteps is None or len(timesteps) == 0 else self.index_for_timestep(timesteps[0])
+        T = self.num_inference_steps if timesteps is None else len(timesteps)
+        rows = [self.step_row(k0 + j, c, p) for j, (c, p) in enumerate(self.step_plan(k0, T, restart))]
+        return torch.tensor(rows, dtype=torch.float32).reshape(-1, UNIPC_ROW)
+
+    def buffers(self, x: torch.Tensor):
+        """(hist, last) for samples shaped like x: reallocated (zeroed), and the solver restarted, when x's shape or device
+        differs from theirs"""
+        R = self.config.solver_order
+        if self.last is None or tuple(self.last.shape) != tuple(x.shape) or self.last.device != x.device:
+            self.hist = torch.zeros((R,) + tuple(x.shape), dtype=torch.float32, device=x.device)
+            self.last = torch.zeros(x.shape, dtype=torch.float32, device=x.device)
+            self._restart()
+        return self.hist, self.last
+
+    def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, return_dict: bool = True,
+             model_output_uncond: Optional[torch.Tensor] = None, guidance_w: float = 0.0,
+             out: Optional[torch.Tensor] = None, **unused):
+        """x at the next timestep of diffusers' UniPC step: the corrector rebuilds `sample` from last_sample (when it runs)
+        and the predictor advances the result.  Deterministic (generator is ignored, as in diffusers).  Extras over
+        diffusers, as in DPMSolverMultistepScheduler.step: `model_output_uncond` + `guidance_w` fuse the classifier-free
+        combine, `out` is the destination (may be `sample`)."""
+        if self.num_inference_steps is None:
+            raise ValueError("Number of inference steps is 'None', you need to run 'set_timesteps' after creating the "
+                             "scheduler")
+        x, eps, eps_u, dst = _step_tensors("UniPCMultistepScheduler.step", model_output, sample, model_output_uncond,
+                                           None, out)
+        if self._step_index is None:
+            self._step_index = self.index_for_timestep(timestep)
+        k = self._step_index
+        hist, last = self.buffers(x)
+        c = self.this_order if self._corrects(k, self._has_last) else 0
+        p = self._order(k, self.lower_order_nums)
+        row = torch.tensor(self.step_row(k, c, p), dtype=torch.float32)
+        n = x.numel()
+        clip = float(self.config.clip_sample_range) if self.config.clip_sample else 0.0
+        with torch.cuda.device(x.device):
+            _ffi.check(_ffi.lib().bg_unipc_step(eps.data_ptr(), _ffi.ptr(eps_u), float(guidance_w), x.data_ptr(),
+                                               dst.data_ptr(), last.data_ptr(), hist.data_ptr(),
+                                               self.config.solver_order, n // x.shape[0], n, row.data_ptr(), clip,
+                                               _ffi.current_stream()), "bg_unipc_step")
+        self.this_order, self._has_last = p, True
         if self.lower_order_nums < self.config.solver_order:
             self.lower_order_nums += 1
         self._step_index += 1

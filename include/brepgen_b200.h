@@ -222,6 +222,33 @@ int bg_dpm_step(const float* eps_cond, const float* eps_uncond, float cfg_w, con
 int bg_dpm_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out, float* hist,
                     uint64_t seed, uint64_t offset0, uint64_t offset_stride, const uint64_t* sample_keys, int64_t per_sample,
                     const int64_t* t_cur, int64_t n, const float* coef_table, const int32_t* step, float clip, void* stream);
+/* UniPC multistep step (diffusers UniPCMultistepScheduler, predict_x0, prediction_type "epsilon", solver_type "bh1" or
+ * "bh2"): the corrector UniC of the previous step's output and the predictor UniP of this one, fp32 with every operation
+ * rounded in diffusers' order.  One row of BG_UNIPC_ROW floats, computed by the host scheduler:
+ *   [0] alpha_s  [1] sigma_s  [2] corrector order c (0 = none, 1..3)  [3] predictor order p (1..3)
+ *   [4] slot_new  [5..7] slots of the x0 of 1, 2, 3 steps back        (small integers stored as floats)
+ *   [8..15]  corrector cc_x, cc_m0, cc_B, r_1, r_2, rho_1, rho_2, rho_t
+ *   [16..22] predictor cp_x, cp_m0, cp_B, r_1, r_2, rho_1, rho_2     [23] unused
+ * Per element, with eps the CFG combine of bg_dpm_step and m_i = hist[slot of i steps back] (slot s = elements s*n ..):
+ *   x0  = clamp((x - sigma_s*eps) / alpha_s, -clip, clip)           (clip <= 0: no clamp)
+ *   xc  = cc_x*last - cc_m0*m_1 - cc_B*(sum_{i<c} rho_i*(m_{i+1} - m_1)/r_i + rho_t*(x0 - m_1))   if c > 0, else x
+ *   last = xc;  hist[slot_new] = x0
+ *   out = cp_x*xc - cp_m0*x0 - cp_B*sum_{i<p} rho_i*(m_i - x0)/r_i
+ * hist is a ring of n_slots slots of n elements; last and hist are read and written in place, out may alias x, and last /
+ * hist alias nothing else.  last == NULL (allowed only with c = 0) skips its store.  per_sample groups the elements as
+ * in the keyed steps; the step draws no noise.  BG_STATUS_BAD_ARG, launching nothing: NULL pointers, n <= 0, per_sample
+ * <= 0 or not dividing n, n_slots outside 1-3, alpha_s <= 0, c outside 0-3 or p outside 1-3, c > 0 without last, a slot
+ * the step uses outside [0, n_slots). */
+#define BG_UNIPC_ROW 24
+int bg_unipc_step(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out, float* last,
+                  float* hist, int32_t n_slots, int64_t per_sample, int64_t n, const float* coef, float clip,
+                  void* stream);
+/* table-driven form for graph capture: the row coef_table[BG_UNIPC_ROW * k .. ] of step k = *step (bg_step_advance), as
+ * written by the host scheduler's coefficient_table (rows are not validated on the device).  last must not be NULL.
+ * Bit-identical to bg_unipc_step with the same row. */
+int bg_unipc_step_tab(const float* eps_cond, const float* eps_uncond, float cfg_w, const float* x, float* out, float* last,
+                      float* hist, int64_t per_sample, int64_t n, const float* coef_table, const int32_t* step, float clip,
+                      void* stream);
 /* Known-token replacement (B-rep completion; runs after the step kernel, in place on x).  x is n fp32 elements in tokens
  * of per_token consecutive elements; token_mask holds one byte per token (n / per_token).  For every element of a token
  * whose byte is non-zero:  x[i] = sqrt_abar*known[i] + sqrt_one_minus_abar*z  (fmaf(sa, known, sb*z); sa*known when
