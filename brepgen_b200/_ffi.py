@@ -65,6 +65,7 @@ SIGNATURES = {
     "bg_repaint_undo_tab": (i32, [vp, i64, i32, u64, vp, i64, vp, vp, vp]),
     "bg_slerp": (i32, [vp, vp, vp, vp, i64, i64, i64, vp, vp]),
     "bg_pndm_step":(i32, [vp, vp, i64, f32, f32, vp, f32, vp, f32, vp, f32, vp, f32, vp]),
+    "bg_cfg_combine": (i32, [vp, vp, vp, vp, i64, i64, i64, vp, vp]),
     "bg_axpby": (i32, [vp, f32, vp, f32, vp, i64, vp]),
     "bg_dedup_surfaces": (i32, [vp, i32, i32, f32, vp, vp, vp]),
     "bg_dedup_edges": (i32, [vp, vp, i32, i32, i32, f32, vp, vp]),

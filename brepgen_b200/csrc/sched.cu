@@ -581,6 +581,62 @@ __global__ void __launch_bounds__(256) pndm_step_kernel(const PndmP p) {
     p.out[i] = p.cs * p.x[i] - p.ce * acc;
   }
 }
+// Per-sample classifier-free combine (mixed-class batches): sample b of eps_c is guided by row uncond_row[b] of eps_u
+// with weight w[b], each operation rounded on its own (the fp32 torch expression pc*(1+w) - pu[row]*w, as dpm_step_kernel
+// and unipc_step_kernel round their fused combine); uncond_row[b] == -1 leaves the sample as it is (copied, or neither
+// read nor written when out aliases eps_c); any other row outside [0, n_uncond) writes NaN.  One thread per group of 4
+// elements of a sample, as launch_grouped; float4 accesses when every row starts 16-byte aligned (vec), else scalar
+// accesses with the sample's last group cut to per_sample % 4 elements.
+struct CfgP {
+  const float *eps_c, *eps_u, *w;
+  const int* row;
+  float* out;
+  long long n_samples, n_uncond, per_sample;
+  bool vec;
+};
+__global__ void __launch_bounds__(256) cfg_combine_kernel(const CfgP p) {
+  const long long gps = (p.per_sample + 3) / 4, ng = p.n_samples * gps;
+  for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += (long long)gridDim.x * blockDim.x) {
+    const long long b = g / gps, q = g - b * gps;
+    const long long r = p.row[b];
+    const long long i0 = b * p.per_sample + q * 4;
+    if (r == -1 && p.out == p.eps_c) continue;
+    const int cnt = (int)min(4ll, p.per_sample - q * 4);
+    float e[4], u[4] = {0.f, 0.f, 0.f, 0.f};
+    const bool bad = r < -1 || r >= p.n_uncond;
+    const float* pu = (r >= 0 && !bad) ? p.eps_u + r * p.per_sample + q * 4 : nullptr;
+    if (p.vec) {
+      const float4 v = *reinterpret_cast<const float4*>(p.eps_c + i0);
+      e[0] = v.x; e[1] = v.y; e[2] = v.z; e[3] = v.w;
+      if (pu) {
+        const float4 y = __ldg(reinterpret_cast<const float4*>(pu));
+        u[0] = y.x; u[1] = y.y; u[2] = y.z; u[3] = y.w;
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        e[j] = j < cnt ? p.eps_c[i0 + j] : 0.f;
+        if (pu && j < cnt) u[j] = pu[j];
+      }
+    }
+    if (bad) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) e[j] = __int_as_float(0x7fc00000);
+    } else if (pu) {
+      const float wb = p.w[b], w1 = __fadd_rn(1.f, wb);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) e[j] = __fsub_rn(__fmul_rn(e[j], w1), __fmul_rn(u[j], wb));
+    }
+    if (p.vec) {
+      *reinterpret_cast<float4*>(p.out + i0) = make_float4(e[0], e[1], e[2], e[3]);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (j < cnt) p.out[i0 + j] = e[j];
+    }
+  }
+}
+
 __global__ void __launch_bounds__(256) axpby_kernel(const float* x, float a, const float* y, float b, float* out, long long n) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
     out[i] = a * x[i] + (y ? b * y[i] : 0.f);
@@ -953,6 +1009,21 @@ int bg_pndm_step(const float* x, float* out, int64_t n, float c_sample, float c_
   p.w[0] = w0; p.w[1] = w1; p.w[2] = w2; p.w[3] = w3;
   pndm_step_kernel<<<grid_for(n), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
   return check_launch("pndm_step_kernel launch");
+}
+
+int bg_cfg_combine(const float* eps_c, const float* eps_u, const int32_t* uncond_row, const float* w, int64_t n_samples,
+                   int64_t n_uncond, int64_t per_sample, float* out, void* stream) {
+  BG_REQUIRE(eps_c && uncond_row && w && out && (eps_u || n_uncond == 0), "cfg_combine: bad arguments");
+  BG_REQUIRE(n_samples > 0 && per_sample > 0 && n_uncond >= 0, "cfg_combine: n_samples and per_sample must be positive, "
+             "n_uncond non-negative");
+  BG_REQUIRE(n_samples <= INT64_MAX / per_sample && n_uncond <= INT64_MAX / per_sample, "cfg_combine: sizes overflow");
+  CfgP p;
+  p.eps_c = eps_c; p.eps_u = eps_u; p.w = w; p.row = uncond_row; p.out = out;
+  p.n_samples = n_samples; p.n_uncond = n_uncond; p.per_sample = per_sample;
+  const auto a16 = [](const void* q) { return q == nullptr || (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+  p.vec = per_sample % 4 == 0 && a16(eps_c) && a16(eps_u) && a16(out);
+  cfg_combine_kernel<<<grid_for(n_samples * ((per_sample + 3) / 4)), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch("cfg_combine_kernel launch");
 }
 
 int bg_axpby(const float* x, float a, const float* y, float b, float* out, int64_t n, void* stream) {

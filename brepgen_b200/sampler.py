@@ -4,7 +4,8 @@ Same stage order, tensor shapes, late face-count increase (sample.py:140-142), c
 (sample.py:46-51,132-134), de-duplication semantics (sample.py:159-183, 242-261), final masking and latent -> grid
 reshapes (sample.py:284-294).  Differences, all result-preserving:
   * no D2H/H2D round trips: dedup runs as device kernels (csrc/dedup.cu), timesteps are device-resident views;
-  * CFG combine is fused into the DDPM update kernel (PNDM steps combine with one bg_axpby);
+  * CFG combine is fused into the DDPM update kernel (PNDM steps combine with one bg_axpby); per-sample guidance
+    (Guidance: a class, w and negative label per sample) combines with bg_cfg_combine before the step;
   * three schedules: "reference" = the shipped PNDM(200)[:158] + DDPM(1000)[-250:] hybrid, "ddpm" = N DDPM steps for
     every stage, which is BASELINE.json's benchmark definition (N = 1000), "ddim" = N DDIM steps for every stage
     (few-step sampling of the same DDPM-trained denoisers), "dpm" = N DPM-Solver++ steps for every stage (the
@@ -21,6 +22,7 @@ no collective on the hot path; `gather_outputs` is the one optional all_gather a
 """
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass, replace
 from typing import Dict, List, Optional, Sequence, Tuple, Union
 
@@ -43,9 +45,12 @@ class CascadeConfig:
     num_surfaces: int = 50               # eval_config.yaml:12 (doubled late for non-CFG runs, sample.py:140-142)
     num_edges: int = 40                  # eval_config.yaml:13
     use_cf: bool = False
-    class_label: int = 0                 # TEXT2INT[...] when use_cf
+    class_label: Union[int, str, Sequence[Union[int, str]]] = 0   # TEXT2INT value or name when use_cf; a sequence: one
+                                                                   # per sample (per-sample guidance, see Guidance)
     bbox_threshold: float = 0.08         # eval_config.yaml:10
-    guidance_w: float = 0.6              # sample.py:49
+    guidance_w: Union[float, Sequence[float]] = 0.6               # sample.py:49; a sequence: one per sample
+    negative_label: Union[int, str, Sequence[Union[int, str]]] = 0  # label of the guidance's second row ("uncond" in
+                                                                     # the reference); a sequence: one per sample
     schedule: str = "reference"          # "reference" | "ddpm" | "ddim" | "dpm" | "unipc" | "repaint"
     ddpm_steps: int = 1000               # per stage, schedule == "ddpm"
     ddim_steps: int = 50                 # per stage, schedule == "ddim"
@@ -137,7 +142,15 @@ def shard_config(cfg: CascadeConfig, global_batch: int, rank: int, world_size: i
         if len(cfg.sample_seeds) != global_batch:
             raise ValueError(f"sample_seeds has {len(cfg.sample_seeds)} entries for a batch of {global_batch}")
         seeds = list(cfg.sample_seeds)[lo:hi]
-    return replace(cfg, noise="per_sample", batch_size=hi - lo, sample_base=cfg.sample_base + lo, sample_seeds=seeds)
+    guided = {}
+    for f in GUIDANCE_FIELDS:     # per-sample guidance fields have the global length, as sample_seeds
+        v = getattr(cfg, f)
+        if _is_seq(v):
+            if len(v) != global_batch:
+                raise ValueError(f"CascadeConfig.{f} has {len(v)} entries for a batch of {global_batch}")
+            guided[f] = list(v)[lo:hi]
+    return replace(cfg, noise="per_sample", batch_size=hi - lo, sample_base=cfg.sample_base + lo, sample_seeds=seeds,
+                   **guided)
 
 
 def per_sample_seeds(cfg: CascadeConfig) -> Optional[List[int]]:
@@ -151,6 +164,140 @@ def per_sample_seeds(cfg: CascadeConfig) -> Optional[List[int]]:
             raise ValueError(f"sample_seeds has {len(cfg.sample_seeds)} entries for batch_size {cfg.batch_size}")
         return [int(s) for s in cfg.sample_seeds]
     return [sample_seed(int(cfg.seed), int(cfg.sample_base) + b) for b in range(cfg.batch_size)]
+
+
+GUIDANCE_FIELDS = ("class_label", "guidance_w", "negative_label")
+
+
+def _is_seq(v) -> bool:
+    return not isinstance(v, (str, bytes)) and (isinstance(v, Sequence) or getattr(v, "ndim", 0) > 0)
+
+
+def _label(v, field: str) -> int:
+    if isinstance(v, str):
+        return TEXT2INT[v]            # an unknown name raises KeyError, as config_from_eval_args does
+    i = int(v)
+    if i != v or not 0 <= i < len(TEXT2INT):
+        raise ValueError(f"CascadeConfig.{field}: label {v!r} is not an integer in [0, {len(TEXT2INT)}) (the class "
+                         "embedding's rows)")
+    return i
+
+
+def per_sample_guidance(cfg: CascadeConfig) -> bool:
+    """True when any of class_label, guidance_w and negative_label is a sequence (one entry per sample)"""
+    return any(_is_seq(getattr(cfg, f)) for f in GUIDANCE_FIELDS)
+
+
+def check_guidance(cfg: CascadeConfig) -> Optional[Tuple[List[int], List[int], List[float]]]:
+    """raises on classifier-free guidance fields cfg cannot run (host checks only: nothing is launched): a sequence whose
+    length is not batch_size, per-sample fields or a non-zero negative_label without use_cf, a label outside [0, 11) (an
+    unknown name raises KeyError), a non-finite guidance_w.  Returns (class labels, negative labels, weights) with one
+    entry per sample (scalars broadcast), or None without use_cf."""
+    if not cfg.use_cf:
+        if per_sample_guidance(cfg):
+            raise ValueError("per-sample class_label, guidance_w or negative_label need a classifier-free model "
+                             "(use_cf=True)")
+        if _label(cfg.negative_label, "negative_label") != 0:
+            raise ValueError(f"negative_label {cfg.negative_label!r} needs a classifier-free model (use_cf=True)")
+        return None
+    B = cfg.batch_size
+    vals = []
+    for f in GUIDANCE_FIELDS:
+        v = getattr(cfg, f)
+        if _is_seq(v):
+            if len(v) != B:
+                raise ValueError(f"CascadeConfig.{f} has {len(v)} entries for batch_size {B}")
+            vals.append(list(v))
+        else:
+            vals.append([v] * B)
+    cls = [_label(v, "class_label") for v in vals[0]]
+    neg = [_label(v, "negative_label") for v in vals[2]]
+    w = [float(v) for v in vals[1]]
+    if not all(math.isfinite(v) for v in w):
+        raise ValueError(f"CascadeConfig.guidance_w must be finite, got {cfg.guidance_w!r}")
+    return cls, neg, w
+
+
+class Guidance:
+    """The classifier-free layout of a denoising loop's forward batch over n samples (n = copies of cfg's batch, e.g. the
+    two designs of an interpolation, each copy guided as its sample):
+      * without CFG the batch is the samples themselves;
+      * scalar fields: the reference's layout, [class]*n + [negative]*n (2n rows), and the step kernels' fused combine
+        with the one w;
+      * per-sample fields (per_sample_guidance): the n conditional rows, then the unconditional row of each guided sample
+        (w_b != 0) in batch order (n + G rows).  bg_cfg_combine combines every guided sample with its row, in place in
+        the conditional half, before the step, which then runs without an uncond input; an unguided sample's eps is its
+        conditional prediction, exactly what e*(1 + 0) - e_u*0 gives, without paying for the forward.
+    Device state (per-sample mode): g (G,) int64 guided samples, uncond_row (n,) int32 (-1 = unguided), w (n,) fp32."""
+
+    def __init__(self, cfg: CascadeConfig, device, n: Optional[int] = None):
+        fields = check_guidance(cfg)
+        self.use_cf = bool(cfg.use_cf)
+        self.per_sample = per_sample_guidance(cfg)
+        self.n = cfg.batch_size if n is None else int(n)
+        self.device = device
+        self.w = cfg.guidance_w                    # the fused kernels' weight (scalar mode; ignored without an uncond)
+        self._labels, self._label = None, None
+        self.G = self.n if self.use_cf else 0
+        if self.per_sample:
+            B = cfg.batch_size
+            if self.n % B:
+                raise ValueError(f"a loop over {self.n} samples is not copies of a batch of {B}")
+            cls, neg, w = (v * (self.n // B) for v in fields)
+            guided = [b for b in range(self.n) if w[b] != 0.0]
+            row = [-1] * self.n
+            for i, b in enumerate(guided):
+                row[b] = i
+            self.G = len(guided)
+            self._labels = cls + [neg[b] for b in guided]
+            self.g = torch.tensor(guided, dtype=torch.int64, device=device)
+            self.uncond_row = torch.tensor(row, dtype=torch.int32, device=device)
+            self.w_dev = torch.tensor(w, dtype=torch.float32, device=device)
+        elif self.use_cf:
+            self._labels = [fields[0][0]] * self.n + [fields[1][0]] * self.n
+        self.rows = self.n + self.G                # rows of the forward batch
+
+    @property
+    def label(self) -> Optional[torch.Tensor]:
+        """(rows, 1) int64 class labels of the forward batch (None without CFG)"""
+        if self._label is None and self._labels is not None:
+            self._label = torch.tensor(self._labels, device=self.device).reshape(-1, 1)
+        return self._label
+
+    def double(self, t: torch.Tensor) -> torch.Tensor:
+        """t (n, ...) -> its rows of the forward batch: t, cat([t, t]) or cat([t, t[g]])"""
+        if not self.use_cf:
+            return t
+        if not self.per_sample:
+            return torch.cat([t, t], 0)
+        return torch.cat([t, t.index_select(0, self.g)], 0) if self.G else t
+
+    def split(self, pred: torch.Tensor):
+        """(eps, eps_uncond or None, w) of a forward batch's prediction for a step kernel.  Per-sample mode combines in
+        place into the conditional half (bg_cfg_combine) and returns no uncond."""
+        if not self.use_cf:
+            return pred, None, self.w
+        if not self.per_sample:
+            n = pred.shape[0] // 2
+            return pred[:n], pred[n:], self.w
+        pc = pred[:self.n]
+        if self.G:
+            if pred.dtype != torch.float32 or not pred.is_contiguous():
+                raise RuntimeError("Guidance.split: the prediction must be contiguous fp32")
+            _ffi.check(_ffi.lib().bg_cfg_combine(pc.data_ptr(), pred[self.n:].data_ptr(), self.uncond_row.data_ptr(),
+                                                self.w_dev.data_ptr(), self.n, self.G, pc[0].numel(), pc.data_ptr(),
+                                                _ffi.current_stream()), "bg_cfg_combine")
+        return pc, None, 0.0
+
+    def eps(self, pred: torch.Tensor) -> torch.Tensor:
+        """the guided eps of a forward batch's prediction, for a step without a fused combine (PNDM)"""
+        pc, pu, w = self.split(pred)
+        if pu is None:
+            return pc
+        eps = torch.empty_like(pc)
+        _ffi.check(_ffi.lib().bg_axpby(pc.data_ptr(), 1.0 + w, pu.data_ptr(), -w, eps.data_ptr(), eps.numel(),
+                                      _ffi.current_stream()), "bg_axpby")
+        return eps
 
 
 def check_schedule(cfg: CascadeConfig) -> None:
@@ -554,6 +701,7 @@ class Cascade:
         lib = _ffi.lib()
         T = len(timesteps)
         B = x.shape[0]
+        guid = Guidance(cfg, dev, B)
         xb = x.detach().float().contiguous().clone()
         n = xb.numel()
         ddim = isinstance(sched, DDIMScheduler)
@@ -591,24 +739,22 @@ class Cascade:
         def body():
             st = _ffi.current_stream()
             _ffi.check(lib.bg_step_advance(ts.data_ptr(), T, step.data_ptr(), t_cur.data_ptr(), st), "bg_step_advance")
-            pred = fwd(torch.cat([xb, xb], 0) if cfg.use_cf else xb, t_cur)
-            pc = pred[:B] if cfg.use_cf else pred
-            pu = pred[B:] if cfg.use_cf else None
+            pc, pu, w = guid.split(fwd(guid.double(xb), t_cur))
             if dpm:
-                _ffi.check(lib.bg_dpm_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(),
+                _ffi.check(lib.bg_dpm_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(w), xb.data_ptr(),
                                                xb.data_ptr(), hist.data_ptr(), seed, off0, stride, _ffi.ptr(keys), n // B,
                                                t_cur.data_ptr(), n, coef.data_ptr(), step.data_ptr(), clip, st),
                            "bg_dpm_step_tab")
             elif unipc:
-                _ffi.check(lib.bg_unipc_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(),
+                _ffi.check(lib.bg_unipc_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(w), xb.data_ptr(),
                                                  xb.data_ptr(), last.data_ptr(), hist.data_ptr(), n // B, n,
                                                  coef.data_ptr(), step.data_ptr(), clip, st), "bg_unipc_step_tab")
             elif ddim:
-                _ffi.check(lib.bg_ddim_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(),
+                _ffi.check(lib.bg_ddim_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(w), xb.data_ptr(),
                                                 xb.data_ptr(), seed, off0, stride, _ffi.ptr(keys), n // B, t_cur.data_ptr(),
                                                 n, coef.data_ptr(), step.data_ptr(), clip, 0, st), "bg_ddim_step_tab")
             else:
-                _ffi.check(lib.bg_ddpm_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(),
+                _ffi.check(lib.bg_ddpm_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(w), xb.data_ptr(),
                                                 xb.data_ptr(), seed, off0, stride, _ffi.ptr(keys), n // B, t_cur.data_ptr(),
                                                 n, coef.data_ptr(), step.data_ptr(), clip, st), "bg_ddpm_step_tab")
             replace(st)
@@ -646,18 +792,20 @@ class Cascade:
     # ------------------------------------------------------------------ one denoising loop
     def _loop(self, cfg: CascadeConfig, sched, timesteps, x, fwd, label2, gen, on_step=None, noise_fn=None, known=None,
               rnoise_fn=None):
-        """fwd(x_in, t_dev) -> eps for a (possibly CFG-doubled) batch; noise_fn(k, shape) -> explicit DDPM / DDIM step noise.
+        """fwd(x_in, t_dev) -> eps for the forward batch of x (Guidance: CFG-doubled, or with the guided samples'
+        unconditional rows; label2 is not read, the forward carries its labels); noise_fn(k, shape) -> explicit DDPM / DDIM
+        step noise.
         known: {slots: (values, token mask)} of a completion: the known tokens are replaced before the first step and after
         every step (sched.replace_known); rnoise_fn(k, shape) -> explicit replacement noise (k = -1 before the first step).
         sched may be self.ddim_inv with its ascending timesteps: a DDIM inversion, run as a DDIM loop that draws nothing."""
-        B = x.shape[0]
+        guid = Guidance(cfg, self.device, x.shape[0])
         k = 0
         fused = isinstance(sched, (DDPMScheduler, DDIMScheduler, DPMSolverMultistepScheduler,   # CFG, noise in the kernel
                                    UniPCMultistepScheduler))
         if known is not None and len(timesteps) > 0:
             x = self._replace(sched, known, x, timesteps[0], -1, rnoise_fn, initial=True)
         if fused and noise_fn is None and rnoise_fn is None and gen is None and len(timesteps) > 0 and \
-                self._use_graph(cfg, len(timesteps), x[0].numel() // x.shape[-1] * B * (2 if cfg.use_cf else 1)):
+                self._use_graph(cfg, len(timesteps), x[0].numel() // x.shape[-1] * guid.rows):
             # on_step (the late face-count increase, sample.py:140-142) changes the shape once: one graph per segment
             lo = 0
             ts_list = [int(t) for t in timesteps]
@@ -686,24 +834,13 @@ class Cascade:
             t_dev = ts_dev[i:i + 1]
             if on_step is not None:
                 x = on_step(int(t), x)
-                B = x.shape[0]
-            if cfg.use_cf:
-                pred = fwd(torch.cat([x, x], 0), t_dev)
-                if fused:
-                    x = self._fused_step(cfg, sched, k, t, x, pred[:B], gen, noise_fn, model_output_uncond=pred[B:],
-                                         guidance_w=cfg.guidance_w)
-                else:
-                    eps = torch.empty_like(x)
-                    w = cfg.guidance_w
-                    _ffi.check(_ffi.lib().bg_axpby(pred[:B].data_ptr(), 1.0 + w, pred[B:].data_ptr(), -w, eps.data_ptr(),
-                                                  eps.numel(), _ffi.current_stream()), "bg_axpby")
-                    x = sched.step(eps, t, x).prev_sample
+            pred = fwd(guid.double(x), t_dev)
+            if fused:
+                pc, pu, w = guid.split(pred)
+                cf = {} if pu is None else dict(model_output_uncond=pu, guidance_w=w)
+                x = self._fused_step(cfg, sched, k, t, x, pc, gen, noise_fn, **cf)
             else:
-                pred = fwd(x, t_dev)
-                if fused:
-                    x = self._fused_step(cfg, sched, k, t, x, pred, gen, noise_fn)
-                else:
-                    x = sched.step(pred, t, x).prev_sample
+                x = sched.step(guid.eps(pred), t, x).prev_sample
             if known is not None:
                 x = self._replace(sched, known, x, t, k, rnoise_fn)
             k += 1
@@ -745,7 +882,8 @@ class Cascade:
         ts = sched.timesteps
         ents = repaint_entries(ts)
         dev = self.device
-        tokens = x[0].numel() // x.shape[-1] * x.shape[0] * (2 if cfg.use_cf else 1)
+        guid = Guidance(cfg, dev, x.shape[0])
+        tokens = x[0].numel() // x.shape[-1] * guid.rows
         if noise_fn is None and unoise_fn is None and len(ents) > 0 and self._use_graph(cfg, len(ents), tokens):
             tables = (sched.coefficient_table().to(dev), sched.undo_table().to(dev),
                       ts.to(device=dev, dtype=torch.int64).contiguous())
@@ -763,17 +901,12 @@ class Cascade:
         for k, (is_step, t) in enumerate(ents):
             if on_step is not None:
                 x = on_step(int(ts[k]), x)
-            B = x.shape[0]
             if is_step:
                 kn, km = known[x.shape[1]] if known is not None else (None, None)
                 nz = noise_fn(k, x.shape).to(dev) if noise_fn is not None else None
-                t_dev = ts_dev[k:k + 1]
-                if cfg.use_cf:
-                    pred = fwd(torch.cat([x, x], 0), t_dev)
-                    x = sched.step(pred[:B], t, x, kn, km, noise=nz, model_output_uncond=pred[B:],
-                                   guidance_w=cfg.guidance_w).prev_sample
-                else:
-                    x = sched.step(fwd(x, t_dev), t, x, kn, km, noise=nz).prev_sample
+                pc, pu, w = guid.split(fwd(guid.double(x), ts_dev[k:k + 1]))
+                cf = {} if pu is None else dict(model_output_uncond=pu, guidance_w=w)
+                x = sched.step(pc, t, x, kn, km, noise=nz, **cf).prev_sample
             else:
                 nz = unoise_fn(k, (sched.undo_transitions,) + tuple(x.shape)).to(dev) if unoise_fn is not None else None
                 x = sched.undo_step(x, t, noise=nz, out=x)
@@ -789,6 +922,7 @@ class Cascade:
         coef, utab, ts = tables
         T = len(ents)
         B = x.shape[0]
+        guid = Guidance(cfg, dev, B)
         xb = x.detach().float().contiguous().clone()
         n = xb.numel()
         step = torch.full((1,), lo - 1, dtype=torch.int32, device=dev)
@@ -805,10 +939,8 @@ class Cascade:
         def step_body():
             st = _ffi.current_stream()
             advance(st)
-            pred = fwd(torch.cat([xb, xb], 0) if cfg.use_cf else xb, t_cur)
-            pc = pred[:B] if cfg.use_cf else pred
-            pu = pred[B:] if cfg.use_cf else None
-            _ffi.check(lib.bg_repaint_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(cfg.guidance_w), xb.data_ptr(),
+            pc, pu, w = guid.split(fwd(guid.double(xb), t_cur))
+            _ffi.check(lib.bg_repaint_step_tab(pc.data_ptr(), _ffi.ptr(pu), float(w), xb.data_ptr(),
                                                xb.data_ptr(), _ffi.ptr(kn), _ffi.ptr(km), xb.shape[-1], s3,
                                                _ffi.ptr(keys), n // B, n, coef.data_ptr(), step.data_ptr(), clip, st),
                        "bg_repaint_step_tab")
@@ -1016,6 +1148,7 @@ class Cascade:
         the RePaint step itself (no separate replacement: replace_noise is not used), and known=None is DDIM with
         resampling."""
         check_schedule(cfg)
+        check_guidance(cfg)
         if source is not None and known is not None:
             raise ValueError("Cascade.run: a variation (source=) cannot be combined with a completion (known=)")
         n_known = check_completion(cfg, known) if known is not None else None
@@ -1046,9 +1179,8 @@ class Cascade:
         S = S0 if cfg.use_cf else 2 * S0
         kn = self._known_tensors(cfg, known, n_known) if known is not None else {}
         cpu_gen = torch.Generator().manual_seed(cfg.seed)             # initial noise: CPU generator (utils.py:62-97)
-        label2 = None
-        if cfg.use_cf:
-            label2 = torch.tensor([cfg.class_label] * B + [TEXT2INT["uncond"]] * B, device=dev).reshape(-1, 1)
+        guid = Guidance(cfg, dev)     # the forward batch of every stage: its labels, and rep2 of the conditioning
+        label2 = guid.label
 
         def noise(name, shape):
             if init_noise is not None and name in init_noise:
@@ -1057,7 +1189,7 @@ class Cascade:
                 return randn_keyed(seeds, self._STAGE_ID[name], shape, dev)
             return torch.randn(shape, generator=cpu_gen).to(dev)
 
-        rep2 = (lambda t: torch.cat([t, t], 0)) if cfg.use_cf else (lambda t: t)
+        rep2 = guid.double
 
         # STEP 1-1 surface positions (sample.py:126-153)
         def late_increase(t, x):
@@ -1087,18 +1219,17 @@ class Cascade:
                 srcs.append(s)
         src = srcs[0] if var else {}
         kept = lambda name: var and tails[name] is None
-        label_inv = None
-        if invert and cfg.use_cf:
-            label_inv = torch.tensor([cfg.class_label] * (len(srcs) * B) + [TEXT2INT["uncond"]] * (len(srcs) * B),
-                                     device=dev).reshape(-1, 1)
+        # the inversion's batch: every source's copy of sample b is inverted under sample b's guidance
+        inv = Guidance(cfg, dev, len(srcs) * B) if invert else None
+        label_inv = inv.label if invert else None
 
         def take(field, maps, scale=1.0):
             # the inversion's conditioning: each source's field gathered through its map (0 where -1), one batch
-            return rep2(torch.cat([torch.where((i >= 0)[..., None], s[field].reshape(-1, s[field].shape[-1])[
+            return inv.double(torch.cat([torch.where((i >= 0)[..., None], s[field].reshape(-1, s[field].shape[-1])[
                 i.long().clamp(min=0)] * scale, 0.0) for s, i in zip(srcs, maps)]))
 
         def holes(maps):
-            return rep2(torch.cat([i < 0 for i in maps]))
+            return inv.double(torch.cat([i < 0 for i in maps]))
 
         def vary(name, shape, maps, scale, model, cond=tuple):
             """maps: one index map per source; model, cond(): the denoiser and its conditioning for an inversion"""

@@ -14,7 +14,7 @@ fp32 torch-CPU operations diffusers uses (SURVEY.md Appendix A.3/A.4).  Device s
 from __future__ import annotations
 
 from types import SimpleNamespace
-from typing import List, Optional
+from typing import List, Optional, Union
 
 import numpy as np
 import torch
@@ -97,6 +97,27 @@ def _step_tensors(what, model_output, sample, model_output_uncond, noise, out):
     eps = model_output.float().contiguous()
     eps_u = None if model_output_uncond is None else model_output_uncond.float().contiguous()
     return x, eps, eps_u, (torch.empty_like(x) if out is None else out)
+
+
+def _guidance(what, eps, eps_u, guidance_w):
+    """(eps, eps_uncond, w) for a step kernel.  A float guidance_w is the kernel's fused combine.  A (B,) fp32 tensor on
+    the sample's device gives each sample its own w (mixed-class batches): bg_cfg_combine with uncond_row = arange(B)
+    writes eps*(1 + w[b]) - eps_uncond*w[b] to a new tensor, and the step runs on it without an uncond input."""
+    if not torch.is_tensor(guidance_w):
+        return eps, eps_u, guidance_w
+    B = eps.shape[0]
+    if tuple(guidance_w.shape) != (B,) or guidance_w.dtype != torch.float32 or guidance_w.device != eps.device:
+        raise RuntimeError(f"{what}: a per-sample guidance_w must be a ({B},) fp32 tensor on {eps.device}, got "
+                           f"{tuple(guidance_w.shape)} {guidance_w.dtype} on {guidance_w.device}")
+    if eps_u is None:
+        raise RuntimeError(f"{what}: a per-sample guidance_w needs model_output_uncond")
+    w = guidance_w.contiguous()
+    rows = torch.arange(B, dtype=torch.int32, device=eps.device)
+    out = torch.empty_like(eps)
+    with torch.cuda.device(eps.device):
+        _ffi.check(_ffi.lib().bg_cfg_combine(eps.data_ptr(), eps_u.data_ptr(), rows.data_ptr(), w.data_ptr(), B, B,
+                                            eps.numel() // B, out.data_ptr(), _ffi.current_stream()), "bg_cfg_combine")
+    return out, None, 0.0
 
 
 def _generator_noise(x: torch.Tensor, generator) -> torch.Tensor:
@@ -309,9 +330,10 @@ class DDPMScheduler(_NoiseStreams):
 
     def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, generator=None, return_dict: bool = True,
              noise: Optional[torch.Tensor] = None, model_output_uncond: Optional[torch.Tensor] = None,
-             guidance_w: float = 0.0, out: Optional[torch.Tensor] = None):
+             guidance_w: Union[float, torch.Tensor] = 0.0, out: Optional[torch.Tensor] = None):
         """x_{t-1}.  Extras over diffusers (all optional): `noise` = explicit N(0,1) tensor (parity runs),
-        `model_output_uncond` + `guidance_w` = classifier-free combine fused into the step (sample.py:134),
+        `model_output_uncond` + `guidance_w` = classifier-free combine fused into the step (sample.py:134; guidance_w
+        may be a (B,) fp32 CUDA tensor, one weight per sample: then bg_cfg_combine runs first, in every scheduler here),
         `out` = destination (may be `sample` for an in-place update).  `generator` may be one generator or, as in
         diffusers, a list with one per batch element (sample i's noise from generator[i]; CPU generators sample on the
         host).  Without `noise` or `generator` the noise comes from the in-kernel stream: batch-wide (set_noise_seed) or
@@ -319,6 +341,7 @@ class DDPMScheduler(_NoiseStreams):
         x, eps, eps_u, dst = _step_tensors("DDPMScheduler.step", model_output, sample, model_output_uncond, noise, out)
         t = _as_int(timestep)
         sb, sa, c_x0, c_x, sigma = self.step_coefficients(t)
+        eps, eps_u, guidance_w = _guidance("DDPMScheduler.step", eps, eps_u, guidance_w)
         noise, seed, offset, keys = self._step_noise(x, sigma != 0.0, noise, generator)
         n = x.numel()
         clip = float(self.config.clip_sample_range) if self.config.clip_sample else 0.0
@@ -413,7 +436,7 @@ class DDIMScheduler(_NoiseStreams):
 
     def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, eta: float = 0.0,
              use_clipped_model_output: bool = False, generator=None, variance_noise: Optional[torch.Tensor] = None,
-             return_dict: bool = True, model_output_uncond: Optional[torch.Tensor] = None, guidance_w: float = 0.0,
+             return_dict: bool = True, model_output_uncond: Optional[torch.Tensor] = None, guidance_w: Union[float, torch.Tensor] = 0.0,
              out: Optional[torch.Tensor] = None):
         """x_{t-1} of diffusers' DDIM step.  When eta > 0 the noise comes from `variance_noise`, else `generator` (one, or
         a list with one per batch element), else the in-kernel stream (per sample after set_sample_keys, else batch-wide),
@@ -427,6 +450,7 @@ class DDIMScheduler(_NoiseStreams):
                              "`generator` or `variance_noise` stays `None`.")
         x, eps, eps_u, dst = _step_tensors("DDIMScheduler.step", model_output, sample, model_output_uncond,
                                            variance_noise, out)
+        eps, eps_u, guidance_w = _guidance("DDIMScheduler.step", eps, eps_u, guidance_w)
         noise, seed, offset, keys = self._step_noise(x, eta > 0, variance_noise, generator)
         n = x.numel()
         with torch.cuda.device(x.device):
@@ -485,7 +509,7 @@ class DDIMInverseScheduler(DDIMScheduler):
         raise NotImplementedError("DDIMInverseScheduler has no known-token replacement")
 
     def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, return_dict: bool = True,
-             model_output_uncond: Optional[torch.Tensor] = None, guidance_w: float = 0.0,
+             model_output_uncond: Optional[torch.Tensor] = None, guidance_w: Union[float, torch.Tensor] = 0.0,
              out: Optional[torch.Tensor] = None):
         """x at level `timestep` from x at the level one step below, and pred_original_sample (the clipped x0 of the
         step).  Extras over diffusers, as in DDIMScheduler.step: `model_output_uncond` + `guidance_w` fuse the
@@ -494,6 +518,7 @@ class DDIMInverseScheduler(DDIMScheduler):
         sb, sa, sa_next, c_dir, _ = self.step_coefficients(t)
         x, eps, eps_u, dst = _step_tensors("DDIMInverseScheduler.step", model_output, sample, model_output_uncond, None,
                                            out)
+        eps, eps_u, guidance_w = _guidance("DDIMInverseScheduler.step", eps, eps_u, guidance_w)
         x0 = torch.empty_like(x)
         n = x.numel()
         clip = float(self.config.clip_sample_range) if self.config.clip_sample else 0.0
@@ -683,7 +708,7 @@ class RePaintScheduler(_NoiseStreams):
 
     def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, original_image: Optional[torch.Tensor],
              mask: Optional[torch.Tensor], generator=None, return_dict: bool = True,
-             model_output_uncond: Optional[torch.Tensor] = None, guidance_w: float = 0.0,
+             model_output_uncond: Optional[torch.Tensor] = None, guidance_w: Union[float, torch.Tensor] = 0.0,
              noise: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None):
         """x at the previous timestep of diffusers' RePaint step: known tokens (mask = 1) at
         sqrt(abar_prev) original_image + sqrt(1 - abar_prev) z, the others the DDIM update with eta = self.eta and the
@@ -702,6 +727,7 @@ class RePaintScheduler(_NoiseStreams):
             kn = original_image.to(device=x.device, dtype=torch.float32).contiguous()
         t = _as_int(timestep)
         coefs = self.step_coefficients(t)
+        eps, eps_u, guidance_w = _guidance("RePaintScheduler.step", eps, eps_u, guidance_w)
         k = self._next_entry()
         if noise is None and generator is not None:
             noise = _generator_noise(x, generator)
@@ -952,7 +978,7 @@ class DPMSolverMultistepScheduler(_NoiseStreams):
 
     def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, generator=None,
              variance_noise: Optional[torch.Tensor] = None, return_dict: bool = True,
-             model_output_uncond: Optional[torch.Tensor] = None, guidance_w: float = 0.0,
+             model_output_uncond: Optional[torch.Tensor] = None, guidance_w: Union[float, torch.Tensor] = 0.0,
              out: Optional[torch.Tensor] = None):
         """x at the next timestep of diffusers' DPM-Solver++ step.  In SDE mode the noise comes from `variance_noise`, else
         `generator` (one, or a list with one per batch element), else the in-kernel stream (per sample after
@@ -965,6 +991,7 @@ class DPMSolverMultistepScheduler(_NoiseStreams):
         sde = self.config.algorithm_type == "sde-dpmsolver++"
         x, eps, eps_u, dst = _step_tensors("DPMSolverMultistepScheduler.step", model_output, sample, model_output_uncond,
                                            variance_noise if sde else None, out)
+        eps, eps_u, guidance_w = _guidance("DPMSolverMultistepScheduler.step", eps, eps_u, guidance_w)
         if self._step_index is None:
             self._step_index = self.index_for_timestep(timestep)
         k = self._step_index
@@ -1191,7 +1218,7 @@ class UniPCMultistepScheduler(_NoiseStreams):
         return self.hist, self.last
 
     def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, return_dict: bool = True,
-             model_output_uncond: Optional[torch.Tensor] = None, guidance_w: float = 0.0,
+             model_output_uncond: Optional[torch.Tensor] = None, guidance_w: Union[float, torch.Tensor] = 0.0,
              out: Optional[torch.Tensor] = None, **unused):
         """x at the next timestep of diffusers' UniPC step: the corrector rebuilds `sample` from last_sample (when it runs)
         and the predictor advances the result.  Deterministic (generator is ignored, as in diffusers).  Extras over
@@ -1202,6 +1229,7 @@ class UniPCMultistepScheduler(_NoiseStreams):
                              "scheduler")
         x, eps, eps_u, dst = _step_tensors("UniPCMultistepScheduler.step", model_output, sample, model_output_uncond,
                                            None, out)
+        eps, eps_u, guidance_w = _guidance("UniPCMultistepScheduler.step", eps, eps_u, guidance_w)
         if self._step_index is None:
             self._step_index = self.index_for_timestep(timestep)
         k = self._step_index

@@ -337,6 +337,17 @@ int bg_slerp(const float* a, const float* b, const float* alpha, const uint8_t* 
  * unused e_i may be NULL with w_i = 0) */
 int bg_pndm_step(const float* x, float* out, int64_t n, float c_sample, float c_eps, const float* e0, float w0,
                  const float* e1, float w1, const float* e2, float w2, const float* e3, float w3, void* stream);
+/* Per-sample classifier-free combine (mixed-class batches, a guidance scale per sample):
+ *   out[b*per_sample + j] = uncond_row[b] < 0 ? eps_c[b*per_sample + j]
+ *                         : eps_c[...]*(1 + w[b]) - eps_u[uncond_row[b]*per_sample + j]*w[b]
+ * in fp32 with 1 + w[b], both products and the difference each rounded on their own (the torch expression
+ * pc*(1 + w[:, None]) - pu[uncond_row]*w[:, None], bit for bit).  uncond_row (n_samples) int32 and w (n_samples) fp32
+ * live on the device, so there is no host synchronisation and the call is graph-capturable.  out may alias eps_c; then
+ * samples with uncond_row[b] == -1 are neither read nor written.  An entry outside [-1, n_uncond) writes NaN for its
+ * sample.  eps_u may be NULL only when n_uncond == 0.  BG_STATUS_BAD_ARG, launching nothing: any other NULL pointer,
+ * n_samples or per_sample <= 0, n_uncond < 0. */
+int bg_cfg_combine(const float* eps_c, const float* eps_u, const int32_t* uncond_row, const float* w, int64_t n_samples,
+                   int64_t n_uncond, int64_t per_sample, float* out, void* stream);
 /* out = a*x + b*y  (y may be NULL); out = eps_cond*(1+w) - eps_uncond*w is bg_axpby(eps_c, 1+w, eps_u, -w) */
 int bg_axpby(const float* x, float a, const float* y, float b, float* out, int64_t n, void* stream);
 

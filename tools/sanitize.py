@@ -62,6 +62,12 @@ run("variation poisoned gather", VA.test_out_of_range_index_poisons_only_its_tok
 run("variation fill", VA.test_fill_index_matches_oracle, 100, 50, True)
 run("variation dedup index", VA.test_dedup_index_keeps_positions_and_mask, "duplicates", 3, 7)
 run("variation bad args", VA.test_bad_arguments_are_rejected_and_launch_nothing)
+import test_gpu_guidance as GU   # noqa: E402
+run("cfg combine", GU.test_combine_is_the_torch_expression_bit_for_bit, 61 * 6, True)
+run("cfg combine", GU.test_combine_is_the_torch_expression_bit_for_bit, 7 * 40 * 18, False)
+run("cfg combine aliased", GU.test_aliased_unguided_samples_are_not_written)
+run("cfg combine poisoned", GU.test_bad_map_entries_write_nan, 60 * 6)
+run("cfg combine bad args", GU.test_bad_arguments_are_rejected_and_launch_nothing)
 if what != "ops-no-res1":
     run("gemm", T.test_gemm, 128 * 170 + 5, 768, 1024, 0, 0, True, True, 0)   # persistent tiles wrap, residual epilogue
 if what == "all":
